@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- samples/sec of the DeepFM Criteo-shape training step (BASELINE.json config 2) on the fused sm_100a
+"""bench.py -- samples/sec of the DeepFM Criteo-shape training step (BASELINE.json config 2) on the fused sm_90a
 sparse path, driven through the product surface: EasyRecEstimator(pipeline_config) built from a protobuf-text config.
 
 Contract: `python bench.py --gpus N --steps K --warmup W` (torchrun for N>1) prints ONE JSON line on rank 0.
@@ -18,6 +18,9 @@ V = 10M, and 100M - the north-star size - when N = 8).
   roofline     the dominant own HBM-bound kernel (K7 = er_embedding_bwd, else K2 = er_embedding_fwd): algorithmic
                bytes (SURVEY.md 8d) / CUDA-event time, L2 flushed between launches, vs MEASURED_PEAKS.json hbm_gbs
   cpu_baseline the CPU oracle port of the same step on a bounded sample (rank 0, N = 1)
+
+`--dump-outputs DIR` writes what the last timed step returned (the loss and the predictions) as DIR/<name>.npy, so
+two builds of the project can be compared output for output: every input is generated from fixed seeds.
 
 `--impl reference` times the CPU oracle port (TensorFlow, hence the real reference, cannot be installed in this
 image: DESIGN.md) with the host threads it runs fastest with, for exactly --steps / --warmup steps (capped at 64).
@@ -62,6 +65,8 @@ def parse():
   ap.add_argument('--no-cpu-baseline', action='store_true')
   ap.add_argument('--no-extras', action='store_true', help='skip the optimizer / file / C3 lines (quick runs)')
   ap.add_argument('--kernel-iters', type=int, default=30)
+  ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                  help='write the loss and predictions of the last timed step as DIR/<name>.npy (float32)')
   return ap.parse_args()
 
 
@@ -69,12 +74,12 @@ def peaks():
   p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
   if os.path.exists(p):
     d = json.load(open(p))
-    return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)', float(d.get('bf16_tflops', 2250.0))
-  return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)', 2250.0
+    return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)', float(d.get('bf16_tflops', 989.0))
+  return 3350.0, 'H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16; not measured)', 989.0
 
 
 class ClockSampler(threading.Thread):
-  """nvidia-smi clocks + throttle reasons during the timed regions (B200_PROFILING.md)."""
+  """nvidia-smi clocks + throttle reasons during the timed regions."""
 
   def __init__(self, index=0):
     super().__init__(daemon=True)
@@ -136,6 +141,18 @@ def algorithmic_bytes(L, S, U, D, k):
 
 
 # --------------------------------------------------------------------------------------
+def dump_outputs(out_dir, loss, probs):
+  """the last timed step's outputs as <name>.npy, float32: loss and probs (a dict of them per task when multi-task)"""
+  os.makedirs(out_dir, exist_ok=True)
+  arrays = {'loss': loss}
+  if isinstance(probs, dict):
+    arrays.update(('probs_%s' % k, v) for k, v in probs.items())
+  else:
+    arrays['probs'] = probs
+  for name, t in arrays.items():
+    np.save(os.path.join(out_dir, name + '.npy'), np.asarray(t.detach().float().cpu().numpy(), np.float32).reshape(-1))
+
+
 def cpu_step_oracle(state, ids, dense, labels, V, B, lr=0.01):
   """One training step of the same DeepFM on the CPU oracle (numpy + oracle/er_oracle.c)."""
   from easyrec_b200 import workloads
@@ -225,16 +242,6 @@ def run_cpu(args, steps, warmup, vocab):
   return B * steps / dt, n, dt
 
 
-def ncu_traffic(kernel_key):
-  """dram bytes per launch of a kernel from the committed ncu summary (profiles/r02_ncu_traffic.json), or None."""
-  p = os.path.join(ROOT, 'profiles', 'r02_ncu_traffic.json')
-  if not os.path.exists(p):
-    return None, None
-  d = json.load(open(p))
-  v = d.get(kernel_key)
-  return (float(v['dram_bytes']), 'profiles/' + v.get('source', 'r02_ncu_traffic.json')) if v else (None, None)
-
-
 def main():
   args = parse()
   if os.environ.get('ER_BENCH_WATCHDOG'):   # dump every thread's Python stack if the run is still going after N seconds
@@ -253,7 +260,7 @@ def main():
   config = {'workload': workload,
             'optimizer': '%s(sparse rows fused in backward)+%s(dense)' % (opt_name[args.optimizer], opt_name[args.optimizer]),
             'built_from': 'EasyRecEstimator(protobuf-text pipeline config: workloads.c2_config_text)',
-            'l2_flush': 'none in the step loop: table+optimizer state %.1f GB >> 126 MB L2, ids rotate over 16 distinct '
+            'l2_flush': 'none in the step loop: table+optimizer state %.1f GB >> 50 MB L2, ids rotate over 16 distinct '
                         'batches; the per-kernel roofline timings flush L2 (256 MB write) before every launch'
             % ((vocab + 13) * 17 * 4 * 2 / 1e9), 'parallelism': '%s%d' % ('ep' if ep else 'dp', world)}
 
@@ -321,7 +328,7 @@ def main():
     """row-sharded runs name the next batch (its id exchange runs beside the current step); None on the last step"""
     return devb[(i + 1) % n_rot][0] if (ep and i + 1 < n) else None
 
-  def timed_resident(est, steps, warm):
+  def timed_resident(est, steps, warm, dump=False):
     """device-resident throughput: CUDA events around `steps` train_step calls"""
     for i in range(warm):
       est.trainer.train_step(*devb[i % n_rot], next_features=nxt(i, warm))
@@ -329,9 +336,11 @@ def main():
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
     for i in range(steps):
-      loss, _ = est.trainer.train_step(*devb[i % n_rot], next_features=nxt(i, steps))
+      loss, probs = est.trainer.train_step(*devb[i % n_rot], next_features=nxt(i, steps))
     ev1.record()
     barrier()
+    if dump and rank == 0:   # before later steps reuse the captured graph's output buffers
+      dump_outputs(args.dump_outputs, loss, probs)
     return max_over_ranks(ev0.elapsed_time(ev1)), float(loss)
 
   def timed_train(est, input_fn, steps, warm):
@@ -355,7 +364,7 @@ def main():
     est.trainer.train_step(*devb[i % n_rot], next_features=nxt(i, W))
   barrier()
   sampler.mark()
-  ms, final_loss = timed_resident(est, args.steps, 0)
+  ms, final_loss = timed_resident(est, args.steps, 0, dump=bool(args.dump_outputs))
   value = world * B * args.steps / (ms / 1000.0)
   per_step_launches = getattr(est.trainer, 'launches_per_step', None)
   if per_step_launches is None:   # eager run: count the launches of one step
@@ -546,9 +555,11 @@ def run_c4(args, rank, world, dev, ep, graph, barrier, max_over_ranks):
   ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
   ev0.record()
   for i in range(steps):
-    loss, _ = est.trainer.train_step(*devb[i % n_rot], next_features=nxt(i, steps))
+    loss, probs = est.trainer.train_step(*devb[i % n_rot], next_features=nxt(i, steps))
   ev1.record()
   barrier()
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, loss, probs)
   ms = max_over_ranks(ev0.elapsed_time(ev1))
   launches = int(lib.er_launch_count() - n0)
   if getattr(est.trainer, 'launches_per_step', None):
@@ -696,14 +707,9 @@ def measure_roofline(args, est, devb, B, dev):
   for k in (k_fwd, k_bwd, k_upd):
     k['frac'] = k['achieved'] / peak
   dom = k_bwd if bwd_ms >= fwd_ms else k_fwd
-  traffic, traffic_src = ncu_traffic('er_embedding_bwd' if dom is k_bwd else 'er_embedding_fwd')
   return {'bound': 'hbm', 'achieved': dom['achieved'], 'peak': peak, 'unit': 'GB/s', 'frac': dom['frac'],
-          'traffic': traffic, 'traffic_source': traffic_src,
           'kernel': dom['kernel'], 'peak_source': peak_src,
-          'kernels': [k_fwd, k_bwd, k_upd, k_gemm],
-          'random_64B_row_ceiling_gbs': 1000.0,
-          'ceiling_note': 'tools/microbench_gather.cu: independent random 64 B row reads reach 15.6 Grows/s '
-                          '(1.0 TB/s of rows) at 320K lookups on this B200, not the 6.57 TB/s copy peak'}
+          'kernels': [k_fwd, k_bwd, k_upd, k_gemm]}
 
 
 if __name__ == '__main__':

@@ -2,7 +2,7 @@
 a DAG of named blocks over feature groups, each block a Keras-style layer, a lambda, a recurrent or a
 repeat wrapper; `concat_blocks` / `output_blocks` select the outputs, `top_mlp` finishes.
 
-The wiring is host-side (done once); the layers run on liber_b200: `MLP` = layers.DenseLayer stack (tcgen05
+The wiring is host-side (done once); the layers run on liber_b200: `MLP` = layers.DenseLayer stack (wgmma
 GEMM + fused batch-norm/activation, layers/keras/blocks.py:33-129), `Cross` = DCN-v2 cross
 `x0 * (W x + b) + x` (layers/keras/interaction.py:249-286), `FM` = the FM kernels
 (layers/keras/interaction.py:24-44), `MMoE` = expert MLPs + the softmax mixture kernel

@@ -1,4 +1,4 @@
-// Shared helpers for liber_b200.so (sm_100a only).
+// Shared helpers for liber_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -33,14 +33,14 @@ inline int fail(int code, const std::string& msg) {
     }                                                                      \
   } while (0)
 
-constexpr int kSmCount = 148;  // B200: 2 dies x 74 SMs
+constexpr int kSmCount = 132;  // H100 SXM
 
 __host__ __device__ inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 inline cudaStream_t as_stream(er_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 
 // Cap a 1-D grid: enough CTAs to cover `work_items` at `per_cta`, rounded so
-// large problems run as whole waves of the 148 SMs (grid-stride loops inside).
+// large problems run as whole waves of the 132 SMs (grid-stride loops inside).
 inline int grid_for(int64_t work_items, int per_cta, int ctas_per_sm) {
   int64_t need = ceil_div(work_items, per_cta);
   int64_t wave = (int64_t)kSmCount * ctas_per_sm;
@@ -67,7 +67,7 @@ __device__ __forceinline__ void st_stream_f4(float4* p, const float4& v) {
 // ---- programmatic dependent launch (PDL) ----------------------------------------------------------
 // The step is a chain of short kernels.  Launched with the programmatic-stream-serialization attribute, a
 // kernel's CTAs may be scheduled while its predecessor is still draining: they run their prologue (barrier /
-// TMEM set-up, index math) and block in er_pdl_wait() until the predecessor has completed and its writes are
+// shared-memory set-up, index math) and block in er_pdl_wait() until the predecessor has completed and its writes are
 // visible - so correctness is exactly stream order, only launch latency and ramp-up overlap.  Every kernel
 // launched through launch_pdl() calls er_pdl_wait() before its first global access and then lets its own
 // successor start launching.  ER_PDL=0 in the environment turns the attribute off (plain launches).

@@ -3,9 +3,9 @@
 // fused into two launches forward and two backward, fp32, deterministic.
 //   tf.layers.batch_normalization defaults: momentum 0.99, epsilon 1e-3, batch statistics in
 //   training with the BIASED variance for both the normalisation and the moving average.
-// The GEMMs are er_gemm (gemm.cu, tcgen05) / er_gemm_small (small_gemm.cu).
+// The GEMMs are er_gemm (gemm.cu, wgmma) / er_gemm_small (small_gemm.cu).
 //
-// Decomposition: 32-column tiles x R row chunks (grid ~ 2 waves of the 148 SMs).  Pass 1 writes
+// Decomposition: 32-column tiles x R row chunks (grid ~ 2 waves of the 132 SMs).  Pass 1 writes
 // per-chunk partial statistics (Welford count/mean/M2, merged with Chan's formula in a fixed order
 // -- no atomics, no E[x^2]-E[x]^2 cancellation); pass 2 re-derives the column statistics from the
 // R partials (R*32 L2 reads per CTA) and streams the tile.  Traffic: fwd 2 reads + 1 write of

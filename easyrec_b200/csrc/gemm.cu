@@ -1,33 +1,36 @@
-// Dense-layer GEMM of the interaction stage on the 5th-gen tensor cores (tcgen05 + TMEM), fp32 in /
-// fp32 out with "3xTF32" operand splitting so logits stay within the 1e-4 budget of an fp32 CPU run:
+// Dense-layer GEMM of the interaction stage on the Hopper tensor cores (wgmma), fp32 in / fp32 out with
+// "3xTF32" operand splitting so logits stay within the 1e-4 budget of an fp32 CPU run:
 //
 //     x = hi + lo,  hi = tf32-rounded x,  lo = x - hi  (exact in fp32)
-//     A.B ~= Alo.Bhi + Ahi.Blo + Ahi.Bhi      (three tcgen05.mma.kind::tf32 per k-step, fp32 accumulate)
+//     A.B ~= Alo.Bhi + Ahi.Blo + Ahi.Bhi      (three wgmma ... .tf32 per k-step, fp32 accumulate)
 //
 // Replaces the library SGEMMs of layers/dnn.py:50-87 (tf.layers.dense forward) and of its gradient
-// (dX = dY.W^T, dW = X^T.dY) with one kernel that reads the operands *as they lie* in HBM:
-//   - an operand whose K index is contiguous (activations in forward/dX, W[in,out] in dX) is staged as a
-//     K-major SWIZZLE_128B tile: 128 rows (M or N) x 32 k
-//   - an operand whose M/N index is contiguous (W[in,out] in forward, X and dY in dW) is staged as an
-//     MN-major SWIZZLE_128B_BASE32B tile (the only MN-major form of 32-bit operands): 4 atoms x 32 k-rows
-//     x 32 elements
-//   both are "128 segments of 128 B", so the producer code and the shared-memory offsets are the same and
-//   no transposed copy of any matrix is ever made.
+// (dX = dY.W^T, dW = X^T.dY) with one kernel that reads the operands *as they lie* in HBM.  wgmma takes
+// 32-bit operands from shared memory only K-major, so every operand tile is staged as a K-major
+// SWIZZLE_128B tile (128 rows of M or N x 32 k = 128 B per row, 16 B chunk ^= row % 8):
+//   - an operand whose K index is contiguous (activations in forward/dX, W[in,out] in dX) is stored with
+//     16 B vector stores, 8 threads per row;
+//   - an operand whose M/N index is contiguous (W[in,out] in forward, X and dY in dW) is transposed on its
+//     way into shared memory: a warp loads 16 k-rows x 8 contiguous M/N elements (full 32 B sectors) and
+//     scatters them with 4 B stores that fall in 32 different banks;
+// so no transposed copy of any matrix is ever made.
 //
-// CTA = 128x128 output tile (one k-slice of it under split-K):
-//   - 8 producer warps: global -> registers -> hi/lo split -> swizzled st.shared into a 3-stage mbarrier ring,
-//     with kPrefetch k-blocks of loads in flight per thread (the first ones are issued before the CTA-wide
-//     set-up sync);
-//   - 1 MMA warp: one lane issues the tcgen05.mma's, tcgen05.commit hands the stage back;
-//   - accumulators in TMEM: 128 lanes x 128 columns for Ahi.Bhi and another 128 columns for the two cross
-//     terms (the tensor core truncates the fp32 accumulator on every accumulate: keeping the small terms
-//     apart brings the error down to an fp32 SGEMM's);
-//   - epilogue (the producer warps): tcgen05.ld both accumulators -> add -> transpose through shared memory ->
-//     4 x 128 B coalesced stores (+ bias); optionally the batch-norm statistics of the output columns
-//     (per-warp shifted sums -> per-tile Welford -> the last CTA of a column tile merges the tiles in order).
+// CTA = 128x128 output tile (one k-slice of it under split-K), 2 warpgroups:
+//   - every thread is a producer: global -> registers -> hi/lo split -> swizzled st.shared into a 3-stage ring,
+//     with kPrefetch k-blocks of loads in flight per thread;
+//   - warpgroup g issues the wgmma's of output rows [64g, 64g+64) asynchronously and keeps one k-block of them
+//     in flight while the CTA stages the next one (wait_group 1 with 3 stages: a stage is rewritten only after
+//     both warpgroups have retired the wgmma's that read it);
+//   - accumulators in registers: one for Ahi.Bhi and one for the two cross terms (the tensor core truncates
+//     the fp32 accumulator on every accumulate: keeping the small terms apart brings the error down to an
+//     fp32 SGEMM's);
+//   - epilogue: both accumulators -> add -> shared-memory tile -> 512 B coalesced row stores (+ bias);
+//     optionally the batch-norm statistics of the output columns (per-half shifted sums -> per-tile Welford ->
+//     the last CTA of a column tile merges the tiles in order).
+// The MMA width NM (16/32/64/128 columns) is a template parameter picked from N, so narrow layers do not pay
+// for 128 columns of tensor-core work.
 // Split-K partials are reduced by a second kernel in a fixed order: results are run-to-run deterministic.
-// The kernel is launched with programmatic dependent launch: everything before er_pdl_wait() (barrier init,
-// TMEM allocation) overlaps the previous kernel's drain.
+// The kernel is launched with programmatic dependent launch: its prologue overlaps the previous kernel's drain.
 #include <algorithm>
 
 #include "common.cuh"
@@ -37,14 +40,14 @@ namespace gemm {
 
 constexpr int BM = 128, BN = 128, BK = 32;
 constexpr int kStages = 3;
-constexpr int kPrefetch = 3;      // k-blocks of global loads in flight per producer thread
-constexpr int kProducerThreads = 256;
-constexpr int kThreads = kProducerThreads + 32;
-constexpr int kTileBytes = 128 * 128;          // 128 segments x 128 B
+constexpr int kPrefetch = 2;      // k-blocks of global loads in flight per thread
+constexpr int kThreads = 256;     // 2 warpgroups
+constexpr int kTileBytes = 128 * 128;          // 128 rows x 128 B
 constexpr int kStageBytes = 4 * kTileBytes;    // A hi, A lo, B hi, B lo
-constexpr int kStatBytes = 4 * 128 * 3 * 4;   // per row-quarter Welford partials of the tile's columns
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* align slack */ + 256 /* barriers */ + kStatBytes;
-constexpr uint32_t kTmemCols = 256;   // [0,128): hi.hi accumulator, [128,256): the two cross terms
+constexpr int kOutPitch = BN + 8;              // floats per row of the staged output tile (conflict-free float2)
+constexpr int kStatFloats = 768;               // per-half Welford partials [2][128][3]; reused by the final merge
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* align slack */ + kStatFloats * 4 + 16;
+static_assert(BM * kOutPitch * 4 <= kStages * kStageBytes, "output tile must fit in the stage ring");
 
 struct Args {
   const float* A;
@@ -66,53 +69,82 @@ struct Args {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("{ .reg .b64 st; mbarrier.arrive.shared::cta.b64 st, [%0]; }" ::"r"(bar) : "memory");
-}
-// Bounded spin: a protocol bug traps instead of hanging the GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  for (uint32_t spin = 0; !ok; ++spin) {
-    asm volatile(
-        "{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (spin > (1u << 28)) __trap();
-  }
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// shared-memory matrix descriptor (tcgen05); segments are 128 B apart in both modes.
-//   K-major : SWIZZLE_128B (16 B chunk ^= row % 8), 8-row groups 1024 B apart (SBO), LBO unused.
-//   MN-major: 32-bit operands only exist as SWIZZLE_128B_BASE32B (32 B chunk ^= k-row % 4): atoms of
-//             4 k-rows x 32 elements, SBO = 512 B between k-atoms, LBO = 4096 B between M/N atoms.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, int mn_major) {
-  const uint32_t lbo = mn_major ? 4096u : 16u, sbo = mn_major ? 512u : 1024u;
+// wgmma shared-memory matrix descriptor of a K-major SWIZZLE_128B tile: 8-row groups 1024 B apart (SBO),
+// LBO unused; a k-step of 8 tf32 moves the start address by 32 B inside the swizzle atom.
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-  d |= (uint64_t)((lbo >> 4) & 0x3fff) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;                      // descriptor version (Blackwell)
-  d |= (uint64_t)(mn_major ? 1 : 2) << 61;     // SWIZZLE_128B_BASE32B : SWIZZLE_128B
+  d |= (uint64_t)1 << 16;                       // LBO (unused for swizzled K-major)
+  d |= (uint64_t)(1024 >> 4) << 32;             // SBO
+  d |= (uint64_t)1 << 62;                       // SWIZZLE_128B
   return d;
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
+// keeps the compiler from moving accumulator accesses across the asynchronous wgmma's
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] += A[64 x 8] . B[N x 8]^T, both K-major in shared memory; d has N / 2 registers per thread.
+__device__ __forceinline__ void wgmma_tf32(float (&d)[8], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7"
+      "}, %8, %9, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(1));
 }
 
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
@@ -121,27 +153,6 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
   lo = x - hi;
 }
 
-// One operand's 128 B segment `seg` (0..127), 16 B chunk `c` (0..7) of the k-block starting at k0.
-//   mn_major == 0: segment = M/N row (mn0+seg), chunk = k0+4c .. +3
-//   mn_major == 1: segment = (atom j = seg/32, k-row k0 + seg%32), chunk = mn0 + 32j + 4c .. +3
-// The load is only ISSUED here (predicated, destination pre-zeroed); elements past the K / MN edge are
-// cleared by mask_chunk at consume time, so nothing touches the registers while the load is in flight.
-__device__ __forceinline__ int chunk_nvalid(int mn_major, int mn0, int mn_end, int k0, int k_end, int seg, int c) {
-  return mn_major ? mn_end - (mn0 + 32 * (seg >> 5) + 4 * c) : k_end - (k0 + 4 * c);
-}
-__device__ __forceinline__ float4 load_chunk(const float* __restrict__ P, long long ld, int mn_major,
-                                             int mn0, int mn_end, int k0, int k_end, int seg, int c) {
-  int row, col, row_end;
-  if (!mn_major) {
-    row = mn0 + seg; row_end = mn_end; col = k0 + 4 * c;
-  } else {
-    row = k0 + (seg & 31); row_end = k_end; col = mn0 + 32 * (seg >> 5) + 4 * c;
-  }
-  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (row < row_end && chunk_nvalid(mn_major, mn0, mn_end, k0, k_end, seg, c) > 0)
-    v = __ldg(reinterpret_cast<const float4*>(P + (long long)row * ld + col));   // pitch % 4 == 0: in bounds
-  return v;
-}
 __device__ __forceinline__ float4 mask_chunk(float4 v, int nvalid) {
   if (nvalid < 4) {
     if (nvalid < 1) v.x = 0.f;
@@ -150,6 +161,56 @@ __device__ __forceinline__ float4 mask_chunk(float4 v, int nvalid) {
     v.w = 0.f;
   }
   return v;
+}
+
+// Which 4 elements thread (warp, lane) moves in pass j (0..3) of a k-block, relative to the tile origin:
+//   K-major : row r = lane/8 + 4*warp + 32*j (M/N), k = 4*(lane%8) .. +3
+//   MN-major: k = 16*(j%2) + lane%16, M/N = 8*(2*warp + j/2) + 4*(lane/16) .. +3
+// In both cases the load is only ISSUED (predicated, destination zeroed); elements past the K / MN edge are
+// cleared by mask_chunk when the registers are consumed.
+struct Pos {
+  int mn, k;   // first element's tile-relative M/N row and k column
+};
+__device__ __forceinline__ Pos pos_of(int mn_major, int warp, int lane, int j) {
+  if (!mn_major) return Pos{(lane >> 3) + 4 * warp + 32 * j, 4 * (lane & 7)};
+  return Pos{8 * (2 * warp + (j >> 1)) + 4 * (lane >> 4), 16 * (j & 1) + (lane & 15)};
+}
+__device__ __forceinline__ int pos_nvalid(int mn_major, Pos p, int mn0, int mn_end, int k0, int k_end) {
+  return mn_major ? mn_end - (mn0 + p.mn) : k_end - (k0 + p.k);
+}
+__device__ __forceinline__ float4 load_pos(const float* __restrict__ P, long long ld, int mn_major, Pos p,
+                                           int mn0, int mn_end, int k0, int k_end) {
+  const int mn = mn0 + p.mn, k = k0 + p.k;
+  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (!mn_major) {
+    if (mn < mn_end && k < k_end) v = __ldg(reinterpret_cast<const float4*>(P + (long long)mn * ld + k));
+  } else {
+    if (k < k_end && mn < mn_end) v = __ldg(reinterpret_cast<const float4*>(P + (long long)k * ld + mn));
+  }
+  return v;   // pitch % 4 == 0 and the first element is valid: the 16 B lie inside the row
+}
+// byte offset of tile element (row, k) in a K-major SWIZZLE_128B tile
+__device__ __forceinline__ uint32_t swz(int row, int k) {
+  return (uint32_t)row * 128u + (uint32_t)((((k >> 2) ^ (row & 7)) << 4) + ((k & 3) << 2));
+}
+// hi / lo of one thread's 4 elements into the tile pair at `hi_tile` (lo tile kTileBytes further)
+__device__ __forceinline__ void store_pos(uint32_t hi_tile, int mn_major, Pos p, float4 v) {
+  float4 hi, lo;
+  split_tf32(v.x, hi.x, lo.x); split_tf32(v.y, hi.y, lo.y);
+  split_tf32(v.z, hi.z, lo.z); split_tf32(v.w, hi.w, lo.w);
+  if (!mn_major) {
+    const uint32_t o = hi_tile + swz(p.mn, p.k);
+    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
+    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o + kTileBytes), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
+  } else {
+    const float h4[4] = {hi.x, hi.y, hi.z, hi.w}, l4[4] = {lo.x, lo.y, lo.z, lo.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const uint32_t o = hi_tile + swz(p.mn + e, p.k);
+      asm volatile("st.shared.f32 [%0], %1;" ::"r"(o), "f"(h4[e]) : "memory");
+      asm volatile("st.shared.f32 [%0], %1;" ::"r"(o + kTileBytes), "f"(l4[e]) : "memory");
+    }
+  }
 }
 
 struct Welford {
@@ -164,339 +225,226 @@ __device__ __forceinline__ void wf_merge(Welford& a, const Welford& b) {   // Ch
   a.n = n;
 }
 
+template <int NM>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tf32x3_kernel(Args a) {
+  constexpr int R = NM / 2;   // accumulator registers per thread
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // SWIZZLE_128B atoms: 1024 B aligned
-  const uint32_t bar_base = smem_base + kStages * kStageBytes;
-  // barriers: full[s] at +8s, empty[s] at +8(kStages+s), accum at +8*2*kStages, tmem ptr after
-  const uint32_t accum_bar = bar_base + 8 * 2 * kStages;
-  const uint32_t tmem_slot = accum_bar + 8;
-  uint32_t* tmem_slot_ptr =
-      reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  int* s_flag = reinterpret_cast<int*>(tmem_slot_ptr + 1);
-  float* s_stats = reinterpret_cast<float*>(smem_raw + (bar_base + 256 - smem_u32(smem_raw)));
+  const uint32_t raw_u32 = smem_u32(smem_raw);
+  const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;   // SWIZZLE_128B atoms: 1024 B aligned
+  uint8_t* base_ptr = smem_raw + (smem_base - raw_u32);
+  float* s_stats = reinterpret_cast<float*>(base_ptr + kStages * kStageBytes);
+  int* s_flag = reinterpret_cast<int*>(s_stats + kStatFloats);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
   const int k_begin = blockIdx.z * a.k_per_slice;
   const int k_end = min(a.K, k_begin + a.k_per_slice);
   const int n_kb = (k_end - k_begin + BK - 1) / BK;
-  // MMA N: the live columns of this tile rounded up to the instruction granularity
-  const int n_eff = min(BN, ((a.N - n0 + 15) >> 4) << 4);
 
-  const int c = tid & 7, srow = tid >> 3;   // 32 segment rows x 8 chunks per pass, 4 passes
-  const uint32_t off_k = (uint32_t)srow * 128u + (uint32_t)((c ^ (srow & 7)) << 4);
-  const uint32_t off_mn = (uint32_t)srow * 128u + (uint32_t)((c ^ ((srow & 3) << 1)) << 4);
-  const uint32_t off_a = a.a_mn ? off_mn : off_k, off_b = a.b_mn ? off_mn : off_k;
-  // kPrefetch k-blocks of global loads stay in flight per thread (register ring) so the ~1 us HBM/L2
-  // latency is paid once per tile, not once per k-block.
+  Pos pa[4], pb[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    pa[j] = pos_of(a.a_mn, warp, lane, j);
+    pb[j] = pos_of(a.b_mn, warp, lane, j);
+  }
+  // kPrefetch k-blocks of global loads stay in flight per thread (register ring) so the HBM/L2 latency is paid
+  // once per tile, not once per k-block.
   float4 va[kPrefetch][4], vb[kPrefetch][4];
   auto issue = [&](int kb, float4 (&xa)[4], float4 (&xb)[4]) {
     const int k0 = k_begin + kb * BK;
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
-      xa[j] = load_chunk(a.A, a.lda, a.a_mn, m0, a.M, k0, k_end, srow + 32 * j, c);
-#pragma unroll
     for (int j = 0; j < 4; ++j) {
-      // segments wholly outside the MMA's N range are never read by the tensor core
-      const bool live = a.b_mn ? (32 * j < n_eff) : (32 * j + srow < n_eff);
-      xb[j] = live ? load_chunk(a.B, a.ldb, a.b_mn, n0, a.N, k0, k_end, srow + 32 * j, c)
-                   : make_float4(0.f, 0.f, 0.f, 0.f);
+      xa[j] = load_pos(a.A, a.lda, a.a_mn, pa[j], m0, a.M, k0, k_end);
+      // B rows past the MMA width are never read by the tensor core
+      xb[j] = pb[j].mn < NM ? load_pos(a.B, a.ldb, a.b_mn, pb[j], n0, a.N, k0, k_end)
+                            : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   };
-  if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(bar_base + 8 * s, kProducerThreads / 32);
-      mbar_init(bar_base + 8 * (kStages + s), 1);
+  auto stage_out = [&](int kb, const float4 (&xa)[4], const float4 (&xb)[4]) {
+    const int k0 = k_begin + kb * BK;
+    const uint32_t st = smem_base + (uint32_t)(kb % kStages) * kStageBytes;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      store_pos(st, a.a_mn, pa[j], mask_chunk(xa[j], pos_nvalid(a.a_mn, pa[j], m0, a.M, k0, k_end)));
+      if (pb[j].mn < NM)
+        store_pos(st + 2 * kTileBytes, a.b_mn, pb[j], mask_chunk(xb[j], pos_nvalid(a.b_mn, pb[j], n0, a.N, k0, k_end)));
     }
-    mbar_init(accum_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kProducerThreads / 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                 "n"(kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // Everything above touches only this CTA's shared / tensor memory and can run while the previous kernel
-  // of the stream drains (programmatic dependent launch); operands are read only after the wait.  The first
-  // k-blocks' loads are issued before the CTA-wide sync so their latency overlaps it.
+  };
+
+  float acc[R], acc2[R];
+#pragma unroll
+  for (int i = 0; i < R; ++i) acc[i] = acc2[i] = 0.f;
+
   er_pdl_wait();
-  if (warp < kProducerThreads / 32) {
 #pragma unroll
-    for (int u = 0; u < kPrefetch; ++u)
-      if (u < n_kb) issue(u, va[u], vb[u]);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = *tmem_slot_ptr;
+  for (int u = 0; u < kPrefetch; ++u)
+    if (u < n_kb) issue(u, va[u], vb[u]);
 
-  if (warp < kProducerThreads / 32) {
-    // ===== producers: HBM/L2 -> registers -> hi/lo -> swizzled smem =====
-    auto stage_out = [&](int kb, const float4 (&xa)[4], const float4 (&xb)[4]) {
-      const int s = kb % kStages;
-      const uint32_t ph = (uint32_t)(kb / kStages) & 1u;
-      mbar_wait(bar_base + 8 * (kStages + s), ph ^ 1u);   // stage free (first lap passes at once)
-      const uint32_t st = smem_base + (uint32_t)s * kStageBytes;
+  for (int kb0 = 0; kb0 < n_kb; kb0 += kPrefetch) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int k0 = k_begin + kb * BK;
-        const float4 xaj = mask_chunk(xa[j], chunk_nvalid(a.a_mn, m0, a.M, k0, k_end, srow + 32 * j, c));
-        const float4 xbj = mask_chunk(xb[j], chunk_nvalid(a.b_mn, n0, a.N, k0, k_end, srow + 32 * j, c));
-        float4 hi, lo;
-        split_tf32(xaj.x, hi.x, lo.x); split_tf32(xaj.y, hi.y, lo.y);
-        split_tf32(xaj.z, hi.z, lo.z); split_tf32(xaj.w, hi.w, lo.w);
-        const uint32_t o = st + off_a + (uint32_t)j * 4096u;
-        const uint32_t ob = st + off_b + (uint32_t)j * 4096u;
-        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
-        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o + kTileBytes), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
-        split_tf32(xbj.x, hi.x, lo.x); split_tf32(xbj.y, hi.y, lo.y);
-        split_tf32(xbj.z, hi.z, lo.z); split_tf32(xbj.w, hi.w, lo.w);
-        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(ob + 2 * kTileBytes), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
-        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(ob + 3 * kTileBytes), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> tensor core
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_base + 8 * s);                   // one arrival per producer warp
-    };
-    for (int kb0 = 0; kb0 < n_kb; kb0 += kPrefetch) {
+    for (int u = 0; u < kPrefetch; ++u) {
+      const int kb = kb0 + u;
+      if (kb < n_kb) {
+        stage_out(kb, va[u], vb[u]);
+        if (kb + kPrefetch < n_kb) issue(kb + kPrefetch, va[u], vb[u]);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> tensor core
+        __syncthreads();
+        const uint32_t st = smem_base + (uint32_t)(kb % kStages) * kStageBytes;
+        const uint32_t a_hi = st + (uint32_t)wg * (64u * 128u), b_hi = st + 2 * kTileBytes;
+        fence_regs(acc);
+        fence_regs(acc2);
+        wgmma_fence();
 #pragma unroll
-      for (int u = 0; u < kPrefetch; ++u) {
-        const int kb = kb0 + u;
-        if (kb < n_kb) {
-          stage_out(kb, va[u], vb[u]);
-          if (kb + kPrefetch < n_kb) issue(kb + kPrefetch, va[u], vb[u]);
+        for (int kk = 0; kk < BK / 8; ++kk) {
+          const uint64_t ahi = make_desc(a_hi + kk * 32), alo = make_desc(a_hi + kTileBytes + kk * 32);
+          const uint64_t bhi = make_desc(b_hi + kk * 32), blo = make_desc(b_hi + kTileBytes + kk * 32);
+          wgmma_tf32(acc2, alo, bhi);
+          wgmma_tf32(acc2, ahi, blo);
+          wgmma_tf32(acc, ahi, bhi);
         }
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_regs(acc);
+        fence_regs(acc2);
       }
     }
-  } else if (lane == 0) {
-    // ===== MMA issuer (one thread) =====
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a.a_mn << 15) |
-                           ((uint32_t)a.b_mn << 16) | ((uint32_t)(n_eff >> 3) << 17) |
-                           ((uint32_t)(BM >> 4) << 24);
-    const uint32_t a_kstep = a.a_mn ? 1024u : 32u, b_kstep = a.b_mn ? 1024u : 32u;   // 8 k per MMA
-    for (int kb = 0; kb < n_kb; ++kb) {
-      const int s = kb % kStages;
-      const uint32_t ph = (uint32_t)(kb / kStages) & 1u;
-      mbar_wait(bar_base + 8 * s, ph);
-      tc_fence_after();
-      const uint32_t st = smem_base + (uint32_t)s * kStageBytes;
-#pragma unroll
-      for (int kk = 0; kk < BK / 8; ++kk) {
-        const uint64_t ahi = make_desc(st + kk * a_kstep, a.a_mn);
-        const uint64_t alo = make_desc(st + kTileBytes + kk * a_kstep, a.a_mn);
-        const uint64_t bhi = make_desc(st + 2 * kTileBytes + kk * b_kstep, a.b_mn);
-        const uint64_t blo = make_desc(st + 3 * kTileBytes + kk * b_kstep, a.b_mn);
-        // The tensor core truncates (not rounds) the fp32 accumulator on every accumulate, a bias of
-        // ~2^-25 of the accumulator per MMA.  The small cross terms go to their own accumulator, so the
-        // main sum sees one accumulate per 8 k instead of three (measured: error 3e-6 -> ~1e-6, the level
-        // of an fp32 SGEMM).
-        umma_tf32(tmem_d + BN, alo, bhi, idesc, (kb | kk) != 0);
-        umma_tf32(tmem_d + BN, ahi, blo, idesc, 1u);
-        umma_tf32(tmem_d, ahi, bhi, idesc, (kb | kk) != 0);
-      }
-      umma_commit(bar_base + 8 * (kStages + s));   // stage reusable once these MMAs have read it
-    }
-    umma_commit(accum_bar);
   }
+  wgmma_wait<0>();
+  fence_regs(acc);
+  fence_regs(acc2);
+  __syncthreads();   // both warpgroups are done with the stage ring: it becomes the output tile
 
-  if (warp < kProducerThreads / 32) {
-    // ===== epilogue: TMEM -> registers -> shared (transpose) -> global =====
-    mbar_wait(accum_bar, 0u);
-    tc_fence_after();
-    const int q = warp & 3, h = warp >> 2;            // TMEM lane quarter (fixed by warp id % 4), column half
-    float* out = a.n_slices > 1 ? a.partials + (long long)blockIdx.z * a.M * a.N : a.C;
-    const long long ldo = a.n_slices > 1 ? (long long)a.N : a.ldc;
-    const bool vec_ok = (ldo & 3) == 0 && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
-    // A thread owns one row x 32 columns of a block; stores straight from registers would put 32 different
-    // rows in every warp store.  Each warp transposes its two 32x32 blocks through 8 KB of the (now idle)
-    // stage-0 buffer - 16 B units, unit ^= row % 8, conflict-free both ways - so a warp store covers 4 rows
-    // x 128 contiguous bytes.
-    const uint32_t wbuf0 = smem_base + (uint32_t)warp * 8192u;
-    const int nv = min(32, a.M - (m0 + 32 * q));     // valid rows of this warp (<= 0: none)
-    // ---- phase 1: accumulators -> shared; column statistics of the staged blocks ----
-#pragma unroll 1
-    for (int cb = 0; cb < 2; ++cb) {
-      const int col0 = h * 64 + cb * 32;
-      if (col0 >= n_eff) break;                        // warp-uniform
-      const uint32_t wbuf = wbuf0 + (uint32_t)cb * 4096u;
-      uint32_t r[32], r2[32];
-      const uint32_t taddr = tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)col0;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-          "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-            "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-            "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-            "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-            "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(taddr)
-          : "memory");
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-          "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-          : "=r"(r2[0]), "=r"(r2[1]), "=r"(r2[2]), "=r"(r2[3]), "=r"(r2[4]), "=r"(r2[5]), "=r"(r2[6]),
-            "=r"(r2[7]), "=r"(r2[8]), "=r"(r2[9]), "=r"(r2[10]), "=r"(r2[11]), "=r"(r2[12]), "=r"(r2[13]),
-            "=r"(r2[14]), "=r"(r2[15]), "=r"(r2[16]), "=r"(r2[17]), "=r"(r2[18]), "=r"(r2[19]), "=r"(r2[20]),
-            "=r"(r2[21]), "=r"(r2[22]), "=r"(r2[23]), "=r"(r2[24]), "=r"(r2[25]), "=r"(r2[26]), "=r"(r2[27]),
-            "=r"(r2[28]), "=r"(r2[29]), "=r"(r2[30]), "=r"(r2[31])
-          : "r"(taddr + (uint32_t)BN)
-          : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  // ===== epilogue: registers -> shared tile [128][kOutPitch] -> global =====
+  float* tile = reinterpret_cast<float*>(base_ptr);
+  {
+    // accumulator fragment: register i of warp w (of the warpgroup) holds row 16w + lane/4 + 8*((i/2)%2),
+    // column 8*(i/4) + 2*(lane%4) + i%2
+    const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t o = wbuf + (uint32_t)lane * 128u + (uint32_t)((j ^ (lane & 7)) << 4);
-        asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o),
-                     "f"(__uint_as_float(r[4 * j]) + __uint_as_float(r2[4 * j])),
-                     "f"(__uint_as_float(r[4 * j + 1]) + __uint_as_float(r2[4 * j + 1])),
-                     "f"(__uint_as_float(r[4 * j + 2]) + __uint_as_float(r2[4 * j + 2])),
-                     "f"(__uint_as_float(r[4 * j + 3]) + __uint_as_float(r2[4 * j + 3]))
-                     : "memory");
-      }
-      __syncwarp();
-      if (a.bn_part) {
-        // column statistics of this warp's 32 rows: lane l walks column l of the staged block (one full row
-        // per ld.shared: conflict-free); two passes (mean, then squared deviations) - no cancellation
-        // one pass of shifted sums (shift = the column's first value, so no E[x^2]-E[x]^2 cancellation)
-        const int sw = lane >> 2, wi = lane & 3;
-        const float* wb = reinterpret_cast<const float*>(smem_raw + (wbuf - smem_u32(smem_raw)));
-        const float shift = wb[(sw << 2) + wi];            // row 0 (unit ^ 0)
-        float sd0 = 0.f, sd1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+    for (int i = 0; i < R; i += 2) {
+      const int row = rbase + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(tile + row * kOutPitch + col) = make_float2(acc[i] + acc2[i], acc[i + 1] + acc2[i + 1]);
+    }
+  }
+  __syncthreads();
+  float* out = a.n_slices > 1 ? a.partials + (long long)blockIdx.z * a.M * a.N : a.C;
+  const long long ldo = a.n_slices > 1 ? (long long)a.N : a.ldc;
+  const bool vec_ok = (ldo & 3) == 0 && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+  const int m_tiles = gridDim.y;
+  const int n_live = min(NM, a.N - n0);
+  // ---- batch-norm statistics: publish this tile's partials and take a ticket BEFORE the big stores, so the
+  // fence only has to cover 1.5 KB of partials ----
+  if (a.bn_part) {
+    // thread = (column tid % 128, row half tid / 128): one pass of shifted sums (shift = the half's first value,
+    // so no E[x^2]-E[x]^2 cancellation), then the two halves merge in order
+    const int cl = tid & 127, half = tid >> 7;
+    const int nv = min(64, a.M - (m0 + 64 * half));   // valid rows of this half (<= 0: none)
+    if (cl < n_live) {
+      const float* tc = tile + (64 * half) * kOutPitch + cl;
+      const float shift = nv > 0 ? tc[0] : 0.f;
+      float sd0 = 0.f, sd1 = 0.f, sq0 = 0.f, sq1 = 0.f;
 #pragma unroll 8
-        for (int rr = 0; rr < 32; rr += 2) {
-          const float v0 = wb[rr * 32 + ((sw ^ (rr & 7)) << 2) + wi] - shift;
-          const float v1 = wb[(rr + 1) * 32 + ((sw ^ ((rr + 1) & 7)) << 2) + wi] - shift;
-          if (rr < nv) { sd0 += v0; sq0 += v0 * v0; }
-          if (rr + 1 < nv) { sd1 += v1; sq1 += v1 * v1; }
-        }
-        const float fn = (float)max(nv, 1);
-        const float sd = sd0 + sd1;
-        const float mean = shift + sd / fn;
-        const float m20 = (sq0 + sq1) - sd * sd / fn, m21 = 0.f;
-        float* sst = s_stats + ((q * BN) + col0 + lane) * 3;
-        sst[0] = (float)max(nv, 0);
-        sst[1] = mean;
-        sst[2] = fmaxf(m20 + m21, 0.f);
+      for (int rr = 0; rr < 64; rr += 2) {
+        const float v0 = tc[rr * kOutPitch] - shift, v1 = tc[(rr + 1) * kOutPitch] - shift;
+        if (rr < nv) { sd0 += v0; sq0 += v0 * v0; }
+        if (rr + 1 < nv) { sd1 += v1; sq1 += v1 * v1; }
       }
+      const float fn = (float)max(nv, 1);
+      const float sd = sd0 + sd1;
+      float* sst = s_stats + (half * 128 + cl) * 3;
+      sst[0] = (float)max(nv, 0);
+      sst[1] = shift + sd / fn;
+      sst[2] = fmaxf((sq0 + sq1) - sd * sd / fn, 0.f);
     }
-    // ---- batch-norm statistics: publish this tile's partials and take a ticket BEFORE the big stores, so
-    // the fence only has to cover 1.5 KB of partials ----
-    const int m_tiles = gridDim.y;
-    if (a.bn_part) {
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // the 8 epilogue warps (the MMA warp is not here)
-      if (tid < n_eff && n0 + tid < a.N) {
-        Welford t = {s_stats[tid * 3], s_stats[tid * 3 + 1], s_stats[tid * 3 + 2]};
-        for (int qq = 1; qq < 4; ++qq) {
-          const float* p = s_stats + ((qq * BN) + tid) * 3;
-          wf_merge(t, Welford{p[0], p[1], p[2]});
-        }
-        float* gp = a.bn_part + ((long long)blockIdx.y * a.N + n0 + tid) * 3;
-        __stcg(gp, t.n); __stcg(gp + 1, t.mean); __stcg(gp + 2, t.m2);
-        __threadfence();
+    __syncthreads();
+    if (tid < n_live) {
+      Welford t = {s_stats[tid * 3], s_stats[tid * 3 + 1], s_stats[tid * 3 + 2]};
+      const float* p = s_stats + (128 + tid) * 3;
+      wf_merge(t, Welford{p[0], p[1], p[2]});
+      float* gp = a.bn_part + ((long long)blockIdx.y * a.N + n0 + tid) * 3;
+      __stcg(gp, t.n); __stcg(gp + 1, t.mean); __stcg(gp + 2, t.m2);
+      __threadfence();
+    }
+    __syncthreads();
+    if (tid == 0) *s_flag = (atomicAdd(a.bn_counter + blockIdx.x, 1u) == (unsigned)(m_tiles - 1));
+  }
+  // ---- shared -> global: a warp stores NM/4 16 B units of a row, rows in turn ----
+  {
+    const bool add_bias = a.bias != nullptr && a.n_slices == 1;
+    constexpr int kUnits = NM / 4;
+#pragma unroll 4
+    for (int i = tid; i < BM * kUnits; i += kThreads) {
+      const int rr = i / kUnits, u = i % kUnits;
+      const int grow = m0 + rr, col = n0 + 4 * u;
+      if (grow >= a.M || col >= a.N) continue;
+      float4 v = *reinterpret_cast<const float4*>(tile + rr * kOutPitch + 4 * u);
+      if (add_bias) {
+        v.x += a.bias[col];
+        if (col + 1 < a.N) v.y += a.bias[col + 1];
+        if (col + 2 < a.N) v.z += a.bias[col + 2];
+        if (col + 3 < a.N) v.w += a.bias[col + 3];
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid == 0) *s_flag = (atomicAdd(a.bn_counter + blockIdx.x, 1u) == (unsigned)(m_tiles - 1));
-    }
-    // ---- phase 2: shared -> global, coalesced ----
-    {
-      const bool add_bias = a.bias != nullptr && a.n_slices == 1;
-      const int u = lane & 7;                          // 16 B unit of the 128 B row segment
-#pragma unroll 1
-      for (int cb = 0; cb < 2; ++cb) {
-        const int col0 = h * 64 + cb * 32;
-        if (col0 >= n_eff) break;
-        const uint32_t wbuf = wbuf0 + (uint32_t)cb * 4096u;
-        const int col = n0 + col0 + 4 * u;
-        float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (add_bias) {
-          if (col < a.N) bv.x = a.bias[col];
-          if (col + 1 < a.N) bv.y = a.bias[col + 1];
-          if (col + 2 < a.N) bv.z = a.bias[col + 2];
-          if (col + 3 < a.N) bv.w = a.bias[col + 3];
-        }
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int rr = it * 4 + (lane >> 3);         // row of this warp's 32
-          const uint32_t o = wbuf + (uint32_t)rr * 128u + (uint32_t)((u ^ (rr & 7)) << 4);
-          float4 v;
-          asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(o));
-          v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-          const int grow = m0 + 32 * q + rr;
-          if (grow < a.M) {
-            float* orow = out + (long long)grow * ldo;
-            if (vec_ok && col + 3 < a.N) {
-              *reinterpret_cast<float4*>(orow + col) = v;
-            } else {
-              if (col < a.N) orow[col] = v.x;
-              if (col + 1 < a.N) orow[col + 1] = v.y;
-              if (col + 2 < a.N) orow[col + 2] = v.z;
-              if (col + 3 < a.N) orow[col + 3] = v.w;
-            }
-          }
-        }
-      }
-    }
-    if (a.bn_part) {
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (*s_flag) {
-        // Last row-tile of this column tile: combine the per-tile (n, mean, M2) of its 128 columns.  Two
-        // threads per column (even / odd tiles), two passes (global mean, then M2 about it) whose loads are
-        // independent - the whole merge costs a few L2 round trips instead of one per tile - fixed order.
-        __threadfence();
-        const int cl2 = tid & 127, half = tid >> 7;
-        const int col = n0 + cl2;
-        const bool live = cl2 < n_eff && col < a.N;
-        float* s_red = s_stats;                           // reuse: [2][128] floats per pass
-        float cnt = 0.f, wsum = 0.f;
-        if (live) {
-#pragma unroll 16
-          for (int mt = half; mt < m_tiles; mt += 2) {
-            const float* gp = a.bn_part + ((long long)mt * a.N + col) * 3;
-            const float n = __ldcg(gp), mu = __ldcg(gp + 1);
-            cnt += n;
-            wsum += n * mu;
-          }
-        }
-        s_red[half * 128 + cl2] = cnt;
-        s_red[256 + half * 128 + cl2] = wsum;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        const float n_tot = s_red[cl2] + s_red[128 + cl2];
-        const float mean_z = (s_red[256 + cl2] + s_red[384 + cl2]) / fmaxf(n_tot, 1.f);
-        float m2 = 0.f;
-        if (live) {
-#pragma unroll 16
-          for (int mt = half; mt < m_tiles; mt += 2) {
-            const float* gp = a.bn_part + ((long long)mt * a.N + col) * 3;
-            const float n = __ldcg(gp), mu = __ldcg(gp + 1), q2 = __ldcg(gp + 2);
-            const float d = mu - mean_z;
-            m2 += q2 + n * d * d;
-          }
-        }
-        s_red[512 + half * 128 + cl2] = m2;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (live && half == 0) {
-          const float mean = mean_z + (a.bn.bias ? a.bn.bias[col] : 0.f);
-          const float var = (s_red[512 + cl2] + s_red[640 + cl2]) / n_tot;   // biased (tf.layers.batch_normalization)
-          a.bn.save_mean[col] = mean;
-          a.bn.save_rstd[col] = 1.0f / sqrtf(var + a.bn.eps);
-          if (a.bn.moving_mean) {
-            a.bn.moving_mean[col] = a.bn.moving_mean[col] * a.bn.momentum + mean * (1.f - a.bn.momentum);
-            a.bn.moving_var[col] = a.bn.moving_var[col] * a.bn.momentum + var * (1.f - a.bn.momentum);
-          }
-        }
-        if (tid == 0) a.bn_counter[blockIdx.x] = 0u;
+      float* orow = out + (long long)grow * ldo;
+      if (vec_ok && col + 3 < a.N) {
+        *reinterpret_cast<float4*>(orow + col) = v;
+      } else {
+        orow[col] = v.x;
+        if (col + 1 < a.N) orow[col + 1] = v.y;
+        if (col + 2 < a.N) orow[col + 2] = v.z;
+        if (col + 3 < a.N) orow[col + 3] = v.w;
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kProducerThreads / 32) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(kTmemCols)
-                 : "memory");
+  if (a.bn_part) {
+    __syncthreads();
+    if (*s_flag) {
+      // Last row-tile of this column tile: combine the per-tile (n, mean, M2) of its columns.  Two threads per
+      // column (even / odd tiles), two passes (global mean, then M2 about it) whose loads are independent - the
+      // whole merge costs a few L2 round trips instead of one per tile - fixed order.
+      __threadfence();
+      const int cl2 = tid & 127, half = tid >> 7;
+      const int col = n0 + cl2;
+      const bool live = cl2 < n_live;
+      float* s_red = s_stats;                           // reuse: [2][128] floats per pass
+      float cnt = 0.f, wsum = 0.f;
+      if (live) {
+#pragma unroll 16
+        for (int mt = half; mt < m_tiles; mt += 2) {
+          const float* gp = a.bn_part + ((long long)mt * a.N + col) * 3;
+          const float n = __ldcg(gp), mu = __ldcg(gp + 1);
+          cnt += n;
+          wsum += n * mu;
+        }
+      }
+      s_red[half * 128 + cl2] = cnt;
+      s_red[256 + half * 128 + cl2] = wsum;
+      __syncthreads();
+      const float n_tot = s_red[cl2] + s_red[128 + cl2];
+      const float mean_z = (s_red[256 + cl2] + s_red[384 + cl2]) / fmaxf(n_tot, 1.f);
+      float m2 = 0.f;
+      if (live) {
+#pragma unroll 16
+        for (int mt = half; mt < m_tiles; mt += 2) {
+          const float* gp = a.bn_part + ((long long)mt * a.N + col) * 3;
+          const float n = __ldcg(gp), mu = __ldcg(gp + 1), q2 = __ldcg(gp + 2);
+          const float d = mu - mean_z;
+          m2 += q2 + n * d * d;
+        }
+      }
+      s_red[512 + half * 128 + cl2] = m2;
+      __syncthreads();
+      if (live && half == 0) {
+        const float mean = mean_z + (a.bn.bias ? a.bn.bias[col] : 0.f);
+        const float var = (s_red[512 + cl2] + s_red[640 + cl2]) / n_tot;   // biased (tf.layers.batch_normalization)
+        a.bn.save_mean[col] = mean;
+        a.bn.save_rstd[col] = 1.0f / sqrtf(var + a.bn.eps);
+        if (a.bn.moving_mean) {
+          a.bn.moving_mean[col] = a.bn.moving_mean[col] * a.bn.momentum + mean * (1.f - a.bn.momentum);
+          a.bn.moving_var[col] = a.bn.moving_var[col] * a.bn.momentum + var * (1.f - a.bn.momentum);
+        }
+      }
+      if (tid == 0) a.bn_counter[blockIdx.x] = 0u;
+    }
   }
 }
 
@@ -515,7 +463,7 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partials, const f
   }
 }
 
-// Split K when the output has too few tiles to occupy the 148 SMs (the dW GEMMs: K = batch).
+// Split K when the output has too few tiles to occupy the SMs (the dW GEMMs: K = batch).
 static void plan(int64_t M, int64_t N, int64_t K, int* n_slices, int* k_per_slice) {
   const int64_t tiles = ceil_div(M, BM) * ceil_div(N, BN);
   const int64_t kblocks = ceil_div(K, BK);
@@ -528,6 +476,19 @@ static void plan(int64_t M, int64_t N, int64_t K, int* n_slices, int* k_per_slic
   const int64_t per = ceil_div(kblocks, s);
   *k_per_slice = (int)(per * BK);
   *n_slices = (int)ceil_div(kblocks, per);
+}
+
+template <int NM>
+static int launch(const Args& a, dim3 grid, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<NM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kSmemBytes);
+    if (e != cudaSuccess) return er::fail(ER_ERR_CUDA, std::string("er_gemm: ") + cudaGetErrorString(e));
+    attr_set = true;
+  }
+  er::launch_pdl(gemm_tf32x3_kernel<NM>, grid, dim3(kThreads), (size_t)kSmemBytes, st, a);
+  return ER_OK;
 }
 
 }  // namespace gemm
@@ -574,16 +535,12 @@ static int gemm_impl(const float* A, int64_t lda, int32_t a_mn_major, const floa
     a.bn_counter = static_cast<unsigned int*>(ws);
     a.bn_part = reinterpret_cast<float*>(static_cast<char*>(ws) + 1024);
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         kSmemBytes);
-    if (e != cudaSuccess) return er::fail(ER_ERR_CUDA, std::string("er_gemm: ") + cudaGetErrorString(e));
-    attr_set = true;
-  }
   cudaStream_t st = er::as_stream(stream);
   dim3 grid((unsigned)er::ceil_div(N, BN), (unsigned)er::ceil_div(M, BM), (unsigned)a.n_slices);
-  er::launch_pdl(gemm_tf32x3_kernel, grid, dim3(kThreads), (size_t)kSmemBytes, st, a);
+  // MMA width: the narrowest of 16/32/64/128 columns that covers N (N > 128: every tile is 128 wide)
+  const int rc = N > 64 ? launch<128>(a, grid, st) : N > 32 ? launch<64>(a, grid, st)
+               : N > 16 ? launch<32>(a, grid, st) : launch<16>(a, grid, st);
+  if (rc != ER_OK) return rc;
   int launches = 1;
   if (a.n_slices > 1) {
     const long long total = (long long)M * N;

@@ -26,8 +26,8 @@ struct SmallGemm {
 // how the K range is cut: outputs are few and K long (the dW form) -> slices of >= 64, about 2 waves of CTAs in all
 ER_SG_HD int64_t small_gemm_slices(int64_t M, int64_t N, int64_t K) {
   const int64_t out_ctas = (M * N + 255) / 256;
-  if (K < 512 || out_ctas >= 148) return 1;
-  int64_t s = (2 * 148 + out_ctas - 1) / out_ctas;
+  if (K < 512 || out_ctas >= 132) return 1;   // 132 = the H100 SXM's SM count
+  int64_t s = (2 * 132 + out_ctas - 1) / out_ctas;
   const int64_t most = K / 64;
   if (s > most) s = most;
   return s < 1 ? 1 : s;

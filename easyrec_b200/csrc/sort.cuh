@@ -9,7 +9,7 @@
 // row.  8-bit digits, ceil(bits(n_rows)/8) passes (3 for a 10M-row arena).
 //
 // Shape of the launches: the batch is cut into ~one tile per SM (<= 160 tiles of
-// 1024 threads x {2,4,8,16} items), so every launch is a single wave of the 148 SMs.
+// 1024 threads x {2,4,8,16} items), so every launch is a single wave of the 132 SMs.
 // P passes -> P + 1 launches, no separate scan kernels:
 //   init_hist_kernel : rows -> (key, pos) pairs + per-tile histogram of digit 0;
 //                      zeroes the histograms of the later passes
@@ -20,7 +20,7 @@
 //                      at the destination with global atomics (counts are order-free, so
 //                      determinism is kept).
 // Working set at the benchmark shapes (<= 1M pairs x 8 B x 2 buffers) is L2
-// resident on B200: the passes are latency-, not HBM-bound.
+// resident (50 MB on the H100): the passes are latency-, not HBM-bound.
 #pragma once
 #include "common.cuh"
 

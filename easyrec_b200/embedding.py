@@ -1,6 +1,6 @@
 """Embedding arenas and the fused lookup / backward-update engine.
 
-B200-first data layout (DESIGN.md "HBM layout"):
+Data layout (DESIGN.md "Data layout in HBM"):
   * every table with the same embedding_dim lives back to back in ONE fp32 arena
     [n_rows, dim] (row = dim*4 bytes, 64 B at dim 16), so a whole feature group -- all
     slots, all tables -- is one gather launch and one dedup+update pipeline;
@@ -69,7 +69,7 @@ class Arena(object):
     interleave=True stores a row and its optimizer state side by side, [w | state0 | state1], in
     one storage matrix: the fused row update then touches ONE 128 B line per row at dim 16 +
     adagrad instead of two 64 B half-lines in different DRAM pages -- measured 1.9x more random
-    read-modify-writes per second on B200 (tools/microbench_gather.cu), while the forward gather of
+    read-modify-writes per second (tools/microbench_gather.cu), while the forward gather of
     the 64 B weight half costs the same as from a dense [V, 16] table."""
     assert self.n_rows > 0
     n_state = {_lib.OPT_SGD: 0, _lib.OPT_ADAGRAD: 1, _lib.OPT_MOMENTUM: 1}.get(opt_kind, 2)

@@ -1,4 +1,4 @@
-"""InputLayer: feature groups -> dense tensors, on the fused sm_100a lookup path.
+"""InputLayer: feature groups -> dense tensors, on the fused sm_90a lookup path.
 
 Mirrors the reference surface
   InputLayer(feature_configs, feature_groups, ..., wide_output_dim)       layers/input_layer.py:33-69

@@ -5,7 +5,7 @@
         training, *biased* variance for both the normalisation and the moving average (2-D
         inputs take TF's non-fused path)
 
-Per layer: er_gemm (tcgen05 tensor cores, 3xTF32 operand split so logits stay within 1e-4 of an fp32
+Per layer: er_gemm (wgmma tensor cores, 3xTF32 operand split so logits stay within 1e-4 of an fp32
 CPU run; forward, dX and dW read X / W[in,out] / dY in place) + liber_b200's fused bias/batch-norm/ReLU
 epilogue (2 launches forward, 2 backward, deterministic statistics).  There is no torch fallback.
 """
@@ -92,7 +92,7 @@ class _DenseBNAct(torch.autograd.Function):
       gk = torch.empty(x.shape[1], gz.shape[1], dtype=torch.float32, device=x.device)
     if ctx.needs_input_grad[0] and x.is_cuda and _OVERLAP_DW_DX:
       # dW (split-K, few tiles) and dX (many tiles) are independent: fork dW onto a side stream so the two
-      # fill the 148 SMs together (captured as a fork/join inside the step's CUDA graph).  Outputs are
+      # fill the 132 SMs together (captured as a fork/join inside the step's CUDA graph).  Outputs are
       # allocated on the main stream; the side stream only launches.
       cur = torch.cuda.current_stream()
       side = _side_stream(x.device)

@@ -1,4 +1,4 @@
-"""Row-sharded embedding tables (model parallel) with all-to-all over NCCL: the B200 counterpart of
+"""Row-sharded embedding tables (model parallel) with all-to-all over NCCL: the GPU counterpart of
 `embedding_parallel_lookup` (compat/feature_column/feature_column.py:248-357) and of the EP half of
 `optimize_loss` (compat/optimizers.py:294-345).
 

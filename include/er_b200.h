@@ -1,5 +1,5 @@
 /*
- * er_b200.h -- C ABI of liber_b200.so: the sm_100a kernels behind EasyRec's
+ * er_b200.h -- C ABI of liber_b200.so: the sm_90a kernels behind EasyRec's
  * sparse-embedding + feature-interaction training path.
  *
  * The reference (alibaba/EasyRec) has NO native ABI on this path: the path is a
@@ -415,7 +415,7 @@ int er_dense_apply(float* params, const float* grads, float* state0, float* stat
                    const er_opt_t* opt, const float* lr_dev, float* reg_loss_out,
                    er_stream_t stream);
 
-/* ---- dense-layer GEMM on the tcgen05 tensor cores (layers/dnn.py:50-87 tf.layers.dense and its
+/* ---- dense-layer GEMM on the Hopper tensor cores (wgmma) (layers/dnn.py:50-87 tf.layers.dense and its
  * gradient): C[M,N] = A(M,K).B(K,N) (+ bias[n]), fp32 in / fp32 accumulate / fp32 out, operands split
  * hi+lo into three TF32 products ("3xTF32", error ~1e-6 relative - inside the 1e-4 logit budget).
  * Operands are read where they lie:

@@ -125,10 +125,8 @@ def test_dlrm_interaction_matches_the_reference_body(itself, with_dense, interac
 
 def test_reference_dlrm_ep_config_builds(monkeypatch):
   """the reference's own EmbeddingParallel test config (model_class DLRM over the packed Parquet criteo form)"""
-  path = '/root/reference/samples/model_config/dlrm_on_criteo_parquet_ep.config'
-  if not os.path.exists(path):
-    pytest.skip('reference tree not mounted')
-  cfg = config_util.get_configs_from_pipeline_file(path)
+  from test_config import reference_config
+  cfg = config_util.get_configs_from_pipeline_file(reference_config('samples/model_config/dlrm_on_criteo_parquet_ep.config'))
   monkeypatch.setenv('ER_PLAN_ONLY', '1')   # (a 10M-row table: the plan is what is checked)
   il, model, opt = builder.build_model(cfg, 64, 'cpu', cpu_generator=torch.Generator().manual_seed(0))
   assert type(model).__name__ == 'DLRM' and builder.embedding_parallel(cfg)

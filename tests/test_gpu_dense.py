@@ -83,7 +83,7 @@ def test_fused_dnn_matches_torch_and_oracle(B, dims, last_plain):
   r32, x32, y32 = make(torch.float32)
   r64, x64, y64 = make(torch.float64)
 
-  # Mine and torch's are two fp32 evaluations with different summation orders (tcgen05 3xTF32 GEMM + tiled
+  # Mine and torch's are two fp32 evaluations with different summation orders (wgmma 3xTF32 GEMM + tiled
   # Welford statistics vs cuBLAS SGEMM + torch reductions); both are measured against float64 and mine may
   # not be worse than torch's fp32 by more than a small factor (bulk: 99.9th percentile; tail: maximum).
   def no_worse(mine, t32, t64, what, factor=4.0):

@@ -1,9 +1,10 @@
-"""GPU: er_gemm (tcgen05 3xTF32 dense-layer GEMM) against a float64 matmul of the same fp32 inputs.
+"""GPU: er_gemm (wgmma 3xTF32 dense-layer GEMM) against a float64 matmul of the same fp32 inputs.
 
 Tolerance: |err| <= 4e-6 * sum_k |a_mk||b_kn| + 1e-30 per element -- 3xTF32 drops terms of relative size
 2^-21; a plain TF32 product would miss this bound by two orders of magnitude, so the test also proves
 the hi/lo split is live.  Covers the three operand layouts of a dense layer (forward, dX, dW), ragged
-M/N/K, pitched views, bias, and the split-K path (deterministic: two runs are bit-identical)."""
+M/N/K, pitched views, bias, and the split-K path (deterministic: two runs are bit-identical).  N picks the MMA width
+(16 / 32 / 64 / 128 columns): every width has a forward and a dW case."""
 import numpy as np
 import pytest
 import torch
@@ -23,7 +24,7 @@ def _check(a, b, got, bias=None):
 
 
 @pytest.mark.parametrize('M,N,K', [(300, 256, 624), (128, 128, 32), (257, 100, 81), (8192, 64, 128), (1000, 16, 8),
-                                   (5, 1024, 40)])
+                                   (5, 1024, 40), (300, 32, 624)])
 def test_forward_layout(M, N, K):
   from easyrec_b200 import kernels as Kn
   g = torch.Generator(device='cuda').manual_seed(M + N + K)
@@ -43,7 +44,8 @@ def test_dx_layout(M, N, K):
   _check(gz, w.t(), Kn.gemm(gz, w.t()))
 
 
-@pytest.mark.parametrize('M,N,K', [(624, 256, 8192), (81, 256, 4100), (256, 128, 300), (64, 1, 1000)])
+@pytest.mark.parametrize('M,N,K', [(624, 256, 8192), (81, 256, 4100), (256, 128, 300), (64, 1, 1000), (64, 24, 1000),
+                                   (96, 48, 3000)])
 def test_dw_layout_and_split_k(M, N, K):
   from easyrec_b200 import kernels as Kn
   g = torch.Generator(device='cuda').manual_seed(2)

@@ -1,8 +1,7 @@
 """CPU, kernel doubles: every reference sample config that the scope check accepts (and whose tables are small enough to
 materialise here) is built through EasyRecEstimator, trains two steps on a DummyInput batch and evaluates its
 eval_config.metrics_set - the reference's own train_eval tests are exit-code smoke runs over the same files
-(easy_rec/python/test/train_eval_test.py).  Needs /root/reference (skipped elsewhere, e.g. on the GPU box)."""
-import glob
+(easy_rec/python/test/train_eval_test.py).  The configs are the stored copies of tests/golden/reference_configs.tar.xz."""
 import os
 
 import numpy as np
@@ -13,21 +12,17 @@ import host_doubles
 from easyrec_b200 import builder
 from easyrec_b200.config import config_util
 from easyrec_b200.input import readers
-
-REF = '/root/reference'
-PATHS = sorted(glob.glob(os.path.join(REF, 'samples/model_config/*.config'))) + \
-    sorted(glob.glob(os.path.join(REF, 'examples/configs/*.config')))
+from test_config import reference_configs
 
 
-@pytest.mark.skipif(not PATHS, reason='reference checkout not mounted')
 @pytest.mark.timeout(900)
 def test_every_accepted_small_reference_config_trains_and_evaluates(monkeypatch):
   from easyrec_b200.estimator import EasyRecEstimator
   host_doubles.install_all(monkeypatch.setattr)
   trained, failed = [], {}
-  for p in PATHS:
+  for p, text in sorted(reference_configs().items()):
     try:
-      cfg = config_util.get_configs_from_pipeline_file(p)
+      cfg = config_util.get_configs_from_pipeline_file(text)
       builder.check_scope(cfg)
       builder.feature_specs(cfg)
     except Exception:

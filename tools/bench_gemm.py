@@ -1,4 +1,4 @@
-"""Time er_gemm (tcgen05 3xTF32) against torch.mm fp32 SGEMM on the dense-layer shapes of the C2 DeepFM step."""
+"""Time er_gemm (wgmma 3xTF32) against torch.mm fp32 SGEMM on the dense-layer shapes of the C2 DeepFM step."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

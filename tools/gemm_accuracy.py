@@ -1,4 +1,4 @@
-"""Error of er_gemm (3xTF32 on tcgen05) vs cuBLAS fp32 SGEMM and single-pass TF32, against float64."""
+"""Error of er_gemm (3xTF32 on wgmma) vs cuBLAS fp32 SGEMM and single-pass TF32, against float64."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,7 +1,7 @@
-// Calibration microbenchmark: how fast can B200 serve random 64-byte (16 x fp32) row reads /
+// Calibration microbenchmark: how fast can the GPU serve random 64-byte (16 x fp32) row reads /
 // read-modify-writes out of a table much larger than L2?  This is the practical ceiling for the
 // gather (K2) and scatter-update (K7) kernels, next to the streaming-copy peak in
-// MEASURED_PEAKS.json.   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/bin/mb_gather tools/microbench_gather.cu
+// MEASURED_PEAKS.json.   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/bin/mb_gather tools/microbench_gather.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
