@@ -511,7 +511,8 @@ static int gemm_impl(const float* A, int64_t lda, int32_t a_mn_major, const floa
   ER_REQUIRE((lda & 3) == 0 && (ldb & 3) == 0, "operand pitch must be a multiple of 4 floats");
   ER_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
              "operands must be 16-byte aligned");
-  ER_REQUIRE(lda >= (a_mn_major ? M : K) - 3 && ldb >= (b_mn_major ? N : K) - 3, "pitch smaller than row");
+  // a pitch shorter than the row would read the next row's first elements as this row's last ones
+  ER_REQUIRE(lda >= (a_mn_major ? M : K) && ldb >= (b_mn_major ? N : K), "pitch smaller than row");
   ER_REQUIRE(ldc >= N, "ldc < N");
   Args a;
   a.A = A; a.B = B; a.C = C; a.bias = bias;

@@ -422,7 +422,8 @@ int er_dense_apply(float* params, const float* grads, float* state0, float* stat
  *   a_mn_major = 0: A is [M, lda] with k contiguous      a_mn_major = 1: A is [K, lda] with m contiguous
  *   b_mn_major = 0: B is [N, ldb] with k contiguous      b_mn_major = 1: B is [K, ldb] with n contiguous
  * so forward (X, W[in,out]) = (0,1), dX (dY, W) = (0,0), dW (X, dY) = (1,1) need no transposed copy.
- * Pitches must be multiples of 4 floats and base pointers 16-byte aligned (K, M, N are free).
+ * Pitches must be multiples of 4 floats and at least the row (lda >= K resp. M, ldb >= K resp. N, ldc >= N),
+ * and base pointers of A and B 16-byte aligned (K, M, N are free; C may be pitched and misaligned).
  * Small-output / long-K problems are split along K; partials go to ws (er_gemm_workspace_bytes) and
  * are summed in a fixed order (deterministic). */
 size_t er_gemm_workspace_bytes(int64_t M, int64_t N, int64_t K);

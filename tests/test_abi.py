@@ -3,6 +3,9 @@ import ctypes
 import os
 import re
 
+import pytest
+import torch
+
 from easyrec_b200 import _lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -35,6 +38,22 @@ def test_invalid_arguments_fail_loudly_without_gpu():
   # null pointers are rejected on the host before any CUDA call
   st = lib.er_fm_fwd(None, 4, 2, 4, 8, None, None)
   assert st == 1 and b'er_fm_fwd' in lib.er_last_error()
+
+
+@pytest.mark.skipif(torch.cuda.is_available(),
+                    reason='placeholder pointers: with a device, test_gpu_gemm checks this on real buffers')
+def test_gemm_refuses_pitch_shorter_than_row_without_gpu():
+  """A pitch that is a multiple of 4 but short of the row (80 for a row of 81) is refused during validation, for
+  either operand and either layout.  The pointers are placeholders, so the test only runs where no device exists:
+  if validation ever admitted the call, the launch would fail for want of a device instead of touching memory."""
+  lib = _lib.load()
+  p = 1 << 20   # 16-byte aligned placeholder address
+  bn = _lib.ErBnStats(None, p, p, None, None, 1e-3, 0.99)
+  for a_mn, b_mn, lda, ldb in [(0, 1, 80, 84), (1, 1, 80, 84), (0, 0, 84, 80), (0, 1, 84, 80)]:
+    st = lib.er_gemm(p, lda, a_mn, p, ldb, b_mn, None, p, 84, 81, 81, 81, None, 0, None)
+    assert st == _lib.ER_ERR_INVALID_ARG and b'pitch smaller than row' in lib.er_last_error()
+    st = lib.er_gemm_bn(p, lda, a_mn, p, ldb, b_mn, p, 84, 81, 81, 81, ctypes.byref(bn), p, 1 << 20, None)
+    assert st == _lib.ER_ERR_INVALID_ARG and b'pitch smaller than row' in lib.er_last_error()
 
 
 def test_product_never_imports_oracle():
