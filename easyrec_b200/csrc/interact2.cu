@@ -268,6 +268,10 @@ __global__ void __launch_bounds__(256)
 
 // ---- DSSM ------------------------------------------------------------------------------------
 // tf.nn.l2_normalize(x, axis=-1): y = x * rsqrt(max(sum x^2, 1e-12))
+// inv_norm of a row clamped by the epsilon: 1/sqrt(1e-12f) rounded to fp32.  The forward stores exactly this
+// constant for clamped rows (not a runtime rsqrtf of 1e-12f, which may differ from it in the last bits), so the
+// backward can tell clamped rows from inv_norm alone.
+constexpr float kL2ClampInv = 1e6f;
 __global__ void __launch_bounds__(256)
     l2norm_fwd_kernel(const float* __restrict__ x, int64_t batch, int dim, float* __restrict__ y,
                       float* __restrict__ inv_norm) {
@@ -277,21 +281,28 @@ __global__ void __launch_bounds__(256)
   float s = 0.f;
   for (int d = lane; d < dim; d += 32) s += x[b * dim + d] * x[b * dim + d];
   s = warp_sum(s);
-  const float inv = rsqrtf(fmaxf(s, 1e-12f));
+  const float inv = s >= 1e-12f ? rsqrtf(s) : kL2ClampInv;   // NaN sums take the clamp, as fmaxf did
   if (lane == 0) inv_norm[b] = inv;
   for (int d = lane; d < dim; d += 32) y[b * dim + d] = x[b * dim + d] * inv;
 }
-// gx = inv * (gy - y * (gy . y))      (for sum x^2 above the 1e-12 clamp)
+// gx = inv * (gy - y * (gy . y)) above the clamp.  Below it max(sum x^2, 1e-12) passes no gradient to the sum, so
+// gx = gy * inv (TF's gradient of the clamped form).  Rows are told apart by inv == kL2ClampInv, which also takes
+// rows whose sum lies at 1e-12f or a few ulp above it, where rsqrtf rounds to the same value (there the two
+// formulas differ by ~|y|^2 ~ 1 and TF's own gradient is discontinuous).
 __global__ void __launch_bounds__(256)
     l2norm_bwd_kernel(const float* __restrict__ y, const float* __restrict__ inv_norm,
                       const float* __restrict__ gy, int64_t batch, int dim, float* __restrict__ gx) {
   const int lane = threadIdx.x & 31;
   const int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (b >= batch) return;
+  const float inv = inv_norm[b];
+  if (inv == kL2ClampInv) {
+    for (int d = lane; d < dim; d += 32) gx[b * dim + d] = gy[b * dim + d] * inv;
+    return;
+  }
   float dot = 0.f;
   for (int d = lane; d < dim; d += 32) dot += gy[b * dim + d] * y[b * dim + d];
   dot = warp_sum(dot);
-  const float inv = inv_norm[b];
   for (int d = lane; d < dim; d += 32) gx[b * dim + d] = inv * (gy[b * dim + d] - y[b * dim + d] * dot);
 }
 
@@ -422,9 +433,12 @@ extern "C" int er_cross_bwd(const float* x0, const float* xl, const float* w, co
   float* part = s_buf + batch;
   cross_bwd_kernel<<<warps_grid(batch), 256, 0, st>>>(x0, w, xw, gout, batch, dim, gx0, gxl, s_buf,
                                                      accumulate_gx0);
-  const int chunks = (int)ceil_div(batch, (int64_t)256);
+  // chunks of 256 rows, or of a multiple of 256 when that would need more than 65535 chunks (the gridDim.y
+  // limit); fewer chunks than er_cross_workspace_bytes counts, and a fixed order for a given batch
+  const int64_t rows_per_chunk = 256 * ceil_div(ceil_div(batch, (int64_t)256), (int64_t)65535);
+  const int chunks = (int)ceil_div(batch, rows_per_chunk);
   dim3 grid((dim + 31) / 32, chunks);
-  colsum_partial_kernel<<<grid, 256, 0, st>>>(xl, s_buf, gout, batch, dim, 256, part);
+  colsum_partial_kernel<<<grid, 256, 0, st>>>(xl, s_buf, gout, batch, dim, (int)rows_per_chunk, part);
   colsum_final_kernel<<<(dim + 255) / 256, 256, 0, st>>>(part, chunks, dim, gw, gb);
   count_launches(3);
   ER_CUDA_LAUNCH_CHECK();

@@ -468,8 +468,9 @@ int er_bn_act_apply(const float* z, const float* bias, const float* gamma, const
                     float* y, er_stream_t stream);
 
 /* sigmoid cross entropy (tf.losses.sigmoid_cross_entropy,
- * builders/loss_builder.py:36-39): loss_sum += sum_b w*(max(x,0)-x*z+log1p(exp(-|x|)))
- * g_logits[b] = w*(sigmoid(x)-z)*inv_count  (inv_count applied by caller=host scalar) */
+ * builders/loss_builder.py:36-39): *loss_out = inv_count * sum_b w*(max(x,0)-x*z+log1p(exp(-|x|)))
+ * (assigned, not added to), probs[b] = sigmoid(x), g_logits[b] = w*(sigmoid(x)-z)*inv_count.
+ * weights NULL: w = 1; loss_out / probs / g_logits NULL: not written.  One CTA, deterministic. */
 int er_sigmoid_ce_fwd_bwd(const float* logits, const float* labels,
                           const float* weights, int64_t batch, float inv_count,
                           float* loss_out, float* probs, float* g_logits,
@@ -516,7 +517,11 @@ int er_mmoe_mix_bwd(const float* probs, const float* experts, const float* gout,
                     float* g_experts, int32_t accumulate_gexperts, er_stream_t stream);
 
 /* ---- DSSM (model/dssm.py:64-71, model/match_model.py:50-69,213-234) ----
- * l2norm: tf.nn.l2_normalize rows.  inbatch_softmax_ce: rows of sim [B, n_cols >= B], the
+ * l2norm: tf.nn.l2_normalize rows, y = x * rsqrt(max(sum x^2, 1e-12)), inv_norm[b] = that rsqrt.  A row with
+ * sum x^2 < 1e-12f gets inv_norm = 1e6f exactly (1/sqrt(1e-12f) in fp32) and the clamped gradient gx = gy*inv_norm;
+ * other rows get gx = inv_norm*(gy - y*(gy.y)).  The backward picks the branch by inv_norm == 1e6f, so rows with
+ * sum x^2 at 1e-12f or a few ulp above it (where rsqrtf also gives 1e6f) take the clamped gradient too.
+ * inbatch_softmax_ce: rows of sim [B, n_cols >= B], the
  * positive of row b is column b, in-batch duplicates of its item id are masked with -1e32,
  * loss_rows[b] = -log(p_bb + 1e-12)*w_b*inv_wsum (sum them for the loss), g_sim = dloss/dsim. */
 int er_l2norm_fwd(const float* x, int64_t batch, int32_t dim, float* y, float* inv_norm,
