@@ -735,13 +735,18 @@ __global__ void __launch_bounds__(256)
   }
   __syncthreads();
   const int n_chunks = s_first[n_segs];
-  // step scalars: a device scalar (lr_dev: already the effective rate), or the caller's hyper-parameter block
-  // (opt.hyper_dev: lr and Adam's beta powers, from which lr_t is formed here), or the struct itself
-  float lr0 = lr_dev ? *lr_dev : opt.lr;
-  if (!lr_dev && opt.hyper_dev) {
-    lr0 = __ldg(opt.hyper_dev + ER_HYPER_LR);
+  // step scalars: a device scalar (lr_dev: already the effective rate), or lr and Adam's beta powers from the
+  // caller's hyper-parameter block (opt.hyper_dev) or else from the struct itself; Adam's lr_t is formed from
+  // those here, the same way for both sources and as er_embedding_bwd / er_sparse_apply form it
+  float lr0;
+  if (lr_dev) {
+    lr0 = *lr_dev;
+  } else {
+    const float* hy = opt.hyper_dev;
+    lr0 = hy ? __ldg(hy + ER_HYPER_LR) : opt.lr;
     if (opt.kind == ER_OPT_LAZY_ADAM || opt.kind == ER_OPT_ADAM_ROWS)
-      lr0 = adam_lr_t_of(lr0, __ldg(opt.hyper_dev + ER_HYPER_BETA1_POWER), __ldg(opt.hyper_dev + ER_HYPER_BETA2_POWER));
+      lr0 = adam_lr_t_of(lr0, hy ? __ldg(hy + ER_HYPER_BETA1_POWER) : opt.beta1_power,
+                         hy ? __ldg(hy + ER_HYPER_BETA2_POWER) : opt.beta2_power);
   }
   float reg = 0.f;
   for (int ch = blockIdx.x; ch < n_chunks; ch += gridDim.x) {

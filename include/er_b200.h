@@ -399,11 +399,14 @@ int er_auc_hist(const float* probs, const float* labels, int64_t n, const float*
 
 /* Dense optimizer over ONE flat parameter buffer (dense apply_gradients,
  * compat/optimizers.py:413-416): g = grad*grad_scale + l2*w, then the adagrad / adam / sgd rule.
- * segs: DEVICE array describing the tensors inside the flat buffers; the step's rate comes from lr_dev
- * (optional device scalar, used as is), else from opt->hyper_dev (lr and Adam's beta powers in device
- * memory, lr_t = lr*sqrt(1-b2^t)/(1-b1^t) formed in the kernel; grad_scale is NOT taken from it: the dense
- * and the sparse gradients scale differently), else from opt->lr, so a captured CUDA graph can follow a
- * schedule; reg_loss_out (optional) += sum l2/2*w^2. */
+ * segs: DEVICE array describing the tensors inside the flat buffers; the step's rate is lr_dev when given
+ * (optional device scalar: the effective rate, used as is, also for Adam).  Otherwise lr and Adam's beta
+ * powers come from opt->hyper_dev (device memory, so a captured CUDA graph can follow a schedule) or, when
+ * that is NULL, from opt->lr, opt->beta1_power and opt->beta2_power; for the Adam kinds the kernel forms
+ * lr_t = lr*sqrt(1-b2^t)/(1-b1^t) from them, as er_embedding_bwd and er_sparse_apply do.  grad_scale always
+ * comes from opt->grad_scale, never from hyper_dev: the dense and the sparse gradients scale differently.
+ * The rate of a segment is that rate times its lr_mult.  reg_loss_out (optional) += sum l2/2*w^2 of the
+ * pre-update weights (float atomics: not bit-reproducible). */
 typedef struct er_dense_seg {
   int64_t offset;
   int64_t n;
