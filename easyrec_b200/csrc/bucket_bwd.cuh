@@ -70,9 +70,6 @@ constexpr size_t kCntBytes = ((size_t)(kMaxBuckets + 1) * 4 + 255) & ~(size_t)25
 constexpr size_t kTicketBytes = 2048 * 4;
 inline size_t zero_place_bytes() { return 2 * kCntBytes + 256; }
 inline size_t zero_call_bytes() { return 256 + kTicketBytes; }
-inline size_t ws_bytes(int64_t n) {
-  return 2 * a256((size_t)n * 8) + zero_place_bytes() + zero_call_bytes() + 3 * kCntBytes + 256;
-}
 // p: 256-byte aligned.  *counters / *tickets receive the per-call zero block.
 inline Ws carve(char* p, int64_t n, int32_t** counters, int32_t** tickets, char** end) {
   Ws w;

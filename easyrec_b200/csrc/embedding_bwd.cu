@@ -1,7 +1,7 @@
 // K7: backward of the gather+pool = gradient dedup + per-row segment sum + fused
 // optimizer row update, in one pipeline with no host sync:
 //
-//   rows[L] --stable radix sort--> (row, lookup) runs --one lane group per run-->
+//   rows[L] --dedup--> (row, lookup) runs: equal rows adjacent, in ascending lookup order
 //   G_row = sum over the run, in ascending lookup order, of coef_l * dL/d(pooled[seg(l)])
 //   row, state <- optimizer(row, state, G_row * grad_scale)          (same kernel)
 //
@@ -11,22 +11,23 @@
 // (acc += g^2; w -= lr*g*rsqrt(acc); acc0 = 0.1, protos/optimizer.proto:79),
 // EP gradient scaling compat/optimizers.py:315-316.
 //
-// Launches per call: P+1 sort launches (sort.cuh) + runs kernel + hot-row kernel.
-//  * runs kernel: a warp scans 32 sorted positions, ballots the run heads and deals the
-//    positions to its dim/4-lane groups; a group prefetches the row and its optimizer state,
-//    sums the run in lookup order (the sort is stable => the order a sequential CPU
-//    segment-sum uses), applies the optimizer, stores.
-//  * runs longer than kLongRun (Zipf-hot ids, 1-row RawFeature tables: run length = B) are
-//    queued as kChunk-lookup work items; the hot-row kernel sums one chunk per CTA (one
-//    lookup per thread, warp shuffles + a fixed-order shared-memory combine), and the CTA that
-//    finishes a run last adds the chunk partials in chunk order and applies the optimizer:
-//    deterministic, no float atomics.
+// Two dedup engines, chosen by the call:
+//  * bucketed (bucket_bwd.cuh + the bk_* kernels below): every table update.  The lookups are hashed into buckets
+//    by row (bk_place, which er_embedding_bwd_presort can run ahead), a warp or a CTA sorts each bucket on
+//    (row, lookup), and the same kernel sums the runs and applies the optimizer.
+//  * radix (sort.cuh + the bwd_runs_* / bwd_scan_* kernels): calls that also emit the deduplicated gradient,
+//    compact and sorted by row (uniq_rows / uniq_grads / n_uniq).  P+1 sort launches + a head-rank scan + runs
+//    kernel + hot-row kernel.  Dims 64 / 128: a warp scans 32 sorted positions, ballots the run heads and deals
+//    them to its dim/4-lane groups, which sum each run in lookup order (the sort is stable); other non-vector
+//    dims: a thread per (position, column), in lookup order; dims 4..32 and 1: a lane per lookup and a segmented
+//    shuffle scan over the warp (a fixed tree, faster at these widths; last-ulp differences to lookup order).
+// Runs longer than kLongRun (radix) or bk::kQueueRun (bucketed) - Zipf-hot ids - are queued as kChunk-lookup work
+// items; the hot-row kernel sums one chunk per CTA (one lookup per thread, warp shuffles + a fixed-order
+// shared-memory combine), and the CTA that finishes a run last adds the chunk partials in chunk order and applies
+// the optimizer: deterministic, no float atomics.
 //
 // HBM traffic per call (algorithmic): L*8 sorted pairs + L*R gathered upstream gradient
 // rows + U*k*R row/state read-modify-write, R = 4*dim, k = 2 (sgd), 4 (adagrad), 6 (adam).
-#include <stdlib.h>
-#include <string.h>
-
 #include "common.cuh"
 #include "scan.cuh"
 #include "slots.cuh"
@@ -71,8 +72,8 @@ struct BwdArgs {
   int32_t* run_done;         // per hot run: chunks finished
   int2* chunk_list;          // per chunk: (run, chunk index)
   float* partials;           // [chunk][dim]
-  // one-row slots (ER_BUCKET_ONE_ROW): their column sums are computed by the CTAs behind the first main_ctas of the
-  // run kernel's grid (or_chunks == 0: none)
+  // one-row slots (ER_BUCKET_ONE_ROW): their column sums are computed by the CTAs behind the first main_ctas of
+  // bk_fused_kernel's grid (or_chunks == 0: none)
   const int64_t* or_rows;
   float* or_partials;        // [n_slots][or_chunks][dim]
   int32_t* or_tickets;       // [n_slots], zero between calls
@@ -236,10 +237,8 @@ __device__ __forceinline__ int64_t run_end(const uint32_t* __restrict__ keys, in
   return hi;
 }
 
-// One thread registers a hot run and its chunks.
-__device__ __forceinline__ void enqueue_long(const BwdArgs& a, int64_t start, int64_t j, uint32_t key) {
-  const int64_t e = run_end(a.keys, j, a.n, key);
-  const int len = (int)(e - start);
+// One thread registers a hot run (sorted positions [start, start + len)) and its chunks.
+__device__ __forceinline__ void enqueue_run(const BwdArgs& a, int64_t start, int len) {
   const int nch = (len + kChunk - 1) / kChunk;
   const int q = atomicAdd(&a.counters[0], 1);
   const int c0 = atomicAdd(&a.counters[1], nch);
@@ -248,14 +247,21 @@ __device__ __forceinline__ void enqueue_long(const BwdArgs& a, int64_t start, in
   for (int c = 0; c < nch; ++c) a.chunk_list[c0 + c] = make_int2(q, c);
 }
 
+// radix engine: the run of `key` that starts at `start` and still goes on at position j
+__device__ __forceinline__ void enqueue_long(const BwdArgs& a, int64_t start, int64_t j, uint32_t key) {
+  enqueue_run(a, start, (int)(run_end(a.keys, j, a.n, key) - start));
+}
+
 // ---- one-row tables (ER_BUCKET_ONE_ROW slots): weighted column sums -----------------------------------------
 // CTA (slot f, chunk c) sums coef_b * g[b, cols of f] over its kOneRowChunk samples: lane groups take samples
 // g, g + G, ... in order, the groups are added in group order, the chunk partials in chunk order by the slot's
 // last CTA, which then applies the optimizer to the row: deterministic.  CTAs of other slots exit at once.
+// Their shared memory is declared at namespace scope: the compiler then places it behind bk_fused_kernel's own
+// shared variables (s_warp at offset 0), the layout that kernel's code was measured with.
+__shared__ __align__(16) float s_or_part[1024];   // vec: G groups x LANES float4; scalar: 256 floats
+__shared__ int s_or_last;
 template <int LANES>
 __device__ __forceinline__ void one_row_cta(const BwdArgs& a, int cta) {
-  __shared__ __align__(16) float s_part[1024];   // vec: G groups x LANES float4; scalar: 256 floats
-  __shared__ int s_last;
   const int f = cta / a.or_chunks, c = cta - f * a.or_chunks;
   const er_slot_t sl = a.slots[f];
   if (sl.bucket_mode != ER_BUCKET_ONE_ROW) return;
@@ -295,30 +301,30 @@ __device__ __forceinline__ void one_row_cta(const BwdArgs& a, int cta) {
       for (int u = 0; u < U; ++u)
         if (use[u]) f4_fma_sep(g, v[u], coef[u]);
     }
-    reinterpret_cast<float4*>(s_part)[grp * LANES + lane] = g;
+    reinterpret_cast<float4*>(s_or_part)[grp * LANES + lane] = g;
     __syncthreads();
     float4 tot = make_float4(0.f, 0.f, 0.f, 0.f);
     if (threadIdx.x < LANES) {
-      for (int q = 0; q < G; ++q) f4_acc(tot, reinterpret_cast<float4*>(s_part)[q * LANES + threadIdx.x]);
+      for (int q = 0; q < G; ++q) f4_acc(tot, reinterpret_cast<float4*>(s_or_part)[q * LANES + threadIdx.x]);
       __stcg(reinterpret_cast<float4*>(a.or_partials + ((int64_t)f * a.or_chunks + c) * dim) + threadIdx.x, tot);
     }
     __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) s_last = (atomicAdd(&a.or_tickets[f], 1) == used_chunks - 1);
+    if (threadIdx.x == 0) s_or_last = (atomicAdd(&a.or_tickets[f], 1) == used_chunks - 1);
     __syncthreads();
-    if (s_last) {
+    if (s_or_last) {
       __threadfence();
       // the chunk partials: fetched in parallel, added in chunk order
       for (int base = 0; base < used_chunks; base += G) {
         const int q = base + grp;
         if (q < used_chunks)
-          reinterpret_cast<float4*>(s_part)[grp * LANES + lane] =
+          reinterpret_cast<float4*>(s_or_part)[grp * LANES + lane] =
               __ldcg(reinterpret_cast<const float4*>(a.or_partials + ((int64_t)f * a.or_chunks + q) * dim) + lane);
         __syncthreads();
         if (threadIdx.x < LANES) {
           if (base == 0) tot = make_float4(0.f, 0.f, 0.f, 0.f);
           const int m = min(G, used_chunks - base);
-          for (int q2 = 0; q2 < m; ++q2) f4_acc(tot, reinterpret_cast<float4*>(s_part)[q2 * LANES + threadIdx.x]);
+          for (int q2 = 0; q2 < m; ++q2) f4_acc(tot, reinterpret_cast<float4*>(s_or_part)[q2 * LANES + threadIdx.x]);
         }
         __syncthreads();
       }
@@ -338,20 +344,20 @@ __device__ __forceinline__ void one_row_cta(const BwdArgs& a, int cta) {
         if (a.seg_scale) coef = __fmul_rn(coef, a.seg_scale[l]);
         g = __fadd_rn(g, __fmul_rn(gbuf[(int64_t)e * sl.out_stride + sl.out_col + col], coef));
       }
-      s_part[threadIdx.x] = g;
+      s_or_part[threadIdx.x] = g;
       __syncthreads();
       if (threadIdx.x == 0) {
         float tot = 0.f;
-        for (int q = 0; q < 256; ++q) tot = __fadd_rn(tot, s_part[q]);
+        for (int q = 0; q < 256; ++q) tot = __fadd_rn(tot, s_or_part[q]);
         __stcg(a.or_partials + ((int64_t)f * a.or_chunks + c) * dim + col, tot);
       }
       __syncthreads();
     }
     __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) s_last = (atomicAdd(&a.or_tickets[f], 1) == used_chunks - 1);
+    if (threadIdx.x == 0) s_or_last = (atomicAdd(&a.or_tickets[f], 1) == used_chunks - 1);
     __syncthreads();
-    if (s_last && (int)threadIdx.x < dim) {
+    if (s_or_last && (int)threadIdx.x < dim) {
       __threadfence();
       float tot = 0.f;
       for (int q = 0; q < used_chunks; ++q)
@@ -359,17 +365,13 @@ __device__ __forceinline__ void one_row_cta(const BwdArgs& a, int cta) {
       apply_scalar(a, row, (int)threadIdx.x, tot, 0);
     }
     __syncthreads();
-    if (s_last && threadIdx.x == 0) a.or_tickets[f] = 0;
+    if (s_or_last && threadIdx.x == 0) a.or_tickets[f] = 0;
   }
 }
 
 // ---- runs, vector rows (dim = 4*LANES) ---------------------------------------------------
 template <int LANES>
 __global__ void __launch_bounds__(256) bwd_runs_vec_kernel(const __grid_constant__ BwdArgs a) {
-  if (a.or_chunks > 0 && (int)blockIdx.x >= a.main_ctas) {   // CTAs behind the run CTAs: one-row column sums
-    one_row_cta<LANES>(a, (int)blockIdx.x - a.main_ctas);
-    return;
-  }
   extern __shared__ __align__(16) unsigned char s_raw[];
   const SlotView sv = load_slots(s_raw, a.slots, a.n_slots);
   constexpr int GROUPS = 32 / LANES;
@@ -445,10 +447,6 @@ __global__ void __launch_bounds__(256) bwd_runs_vec_kernel(const __grid_constant
 // the last ulp).
 template <int LANES>
 __global__ void __launch_bounds__(256) bwd_scan_vec_kernel(const __grid_constant__ BwdArgs a) {
-  if (a.or_chunks > 0 && (int)blockIdx.x >= a.main_ctas) {   // CTAs behind the run CTAs: one-row column sums
-    one_row_cta<LANES>(a, (int)blockIdx.x - a.main_ctas);
-    return;
-  }
   extern __shared__ __align__(16) unsigned char s_raw[];
   const SlotView sv = load_slots(s_raw, a.slots, a.n_slots);
   constexpr int D4 = LANES;            // float4 per row
@@ -696,10 +694,6 @@ __global__ void __launch_bounds__(256) bwd_long_vec_kernel(const __grid_constant
 
 // ---- scalar rows (wide dim=1 tables, odd dims): one thread per (sorted position, column) ----
 __global__ void __launch_bounds__(256) bwd_runs_scalar_kernel(const __grid_constant__ BwdArgs a) {
-  if (a.or_chunks > 0 && (int)blockIdx.x >= a.main_ctas) {   // CTAs behind the run CTAs: one-row column sums
-    one_row_cta<0>(a, (int)blockIdx.x - a.main_ctas);
-    return;
-  }
   extern __shared__ __align__(16) unsigned char s_raw[];
   const SlotView sv = load_slots(s_raw, a.slots, a.n_slots);
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -779,10 +773,6 @@ __global__ void __launch_bounds__(256) bwd_long_scalar_kernel(const __grid_const
 // Same window protocol as bwd_scan_vec_kernel; a "row" is one float (+ its optimizer slots, which the
 // interleaved arena keeps in the same 32-byte sector), so every tail lane does its own RMW.
 __global__ void __launch_bounds__(256) bwd_scan_d1_kernel(const __grid_constant__ BwdArgs a) {
-  if (a.or_chunks > 0 && (int)blockIdx.x >= a.main_ctas) {   // CTAs behind the run CTAs: one-row column sums
-    one_row_cta<0>(a, (int)blockIdx.x - a.main_ctas);
-    return;
-  }
   extern __shared__ __align__(16) unsigned char s_raw[];
   const SlotView sv = load_slots(s_raw, a.slots, a.n_slots);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -872,15 +862,6 @@ struct BkArgs {
   int warp_ctas;   // CTAs of the warp role (one warp per bucket), 0 in CTA mode
   int med_ctas;    // CTAs of the medium role (they walk med_list)
 };
-
-__device__ __forceinline__ void enqueue_run(const BwdArgs& a, int64_t start, int len) {
-  const int nch = (len + kChunk - 1) / kChunk;
-  const int q = atomicAdd(&a.counters[0], 1);
-  const int c0 = atomicAdd(&a.counters[1], nch);
-  a.long_list[q] = make_int4((int)start, len, c0, nch);
-  a.run_done[q] = 0;
-  for (int c = 0; c < nch; ++c) a.chunk_list[c0 + c] = make_int2(q, c);
-}
 
 // Sum entries [j0, j1) of the sorted pairs `sp` (shared memory) for one row, sequentially in lookup order.
 template <int LANES>
@@ -1546,13 +1527,8 @@ inline int64_t max_long_runs(int64_t n) { return n / kLongRun + 1; }
 inline int64_t max_chunks(int64_t n) { return n / kChunk + max_long_runs(n) + 1; }
 inline int64_t max_one_row_parts(int64_t n) { return n / bk::kOneRowChunk + 2048 + 1; }
 
-inline size_t bwd_ws_bytes(int64_t n, int dim) {
-  return a256((size_t)n * 4) * 3 + a256((size_t)max_long_runs(n) * 16) + a256((size_t)max_long_runs(n) * 4) +
-         a256((size_t)max_chunks(n) * 8) + a256((size_t)max_chunks(n) * dim * 4) +
-         a256(rsort::workspace_bytes(n)) + a256(scan::workspace_bytes(n)) + bk::ws_bytes(n) +
-         a256((size_t)max_one_row_parts(n) * dim * 4) + 512;
-}
-inline BwdWs bwd_carve(void* ws, int64_t n, int dim) {
+// The workspace layout: parts carved from `ws` aligned up to 256 bytes; *end receives the end of the last part.
+inline BwdWs bwd_carve(void* ws, int64_t n, int dim, char** end = nullptr) {
   char* p = reinterpret_cast<char*>(a256(reinterpret_cast<size_t>(ws)));
   BwdWs w;
   w.keys = reinterpret_cast<uint32_t*>(p); p += a256((size_t)n * 4);
@@ -1565,34 +1541,50 @@ inline BwdWs bwd_carve(void* ws, int64_t n, int dim) {
   w.bk = bk::carve(p, n, &w.counters, &w.tickets, &p);
   w.one_row_partials = reinterpret_cast<float*>(p); p += a256((size_t)max_one_row_parts(n) * dim * 4);
   w.sort_ws = p; p += a256(rsort::workspace_bytes(n));
-  w.scan_ws = p;
+  w.scan_ws = p; p += a256(scan::workspace_bytes(n));
+  if (end) *end = p;
   return w;
 }
 
-static bool k7_radix_forced() {
-  static const bool on = [] {
-    const char* e = getenv("ER_K7");
-    return e && strcmp(e, "radix") == 0;
-  }();
-  return on;
+// the layout carved from a null base, plus 768 bytes of slack (aligning the caller's base takes at most 255)
+inline size_t bwd_ws_bytes(int64_t n, int dim) {
+  char* end;
+  bwd_carve(nullptr, n, dim, &end);
+  return reinterpret_cast<size_t>(end) + 768;
 }
 
 static float adam_lr_t(const er_opt_t& o) { return adam_lr_t_of(o.lr, o.beta1_power, o.beta2_power); }
 
+// the hot-row kernel of both engines: sums the queued runs chunk by chunk and applies them
 template <int LANES>
-static void launch_vec(const BwdArgs& a, cudaStream_t st) {
+static void launch_long(const BwdArgs& a, cudaStream_t st) {
+  const size_t sl = slot_smem_bytes(a.n_slots);
+  if constexpr (LANES > 0) {
+    constexpr int TPE = (LANES <= 8) ? 1 : LANES;
+    const size_t smem_long = ((sl + 15) & ~(size_t)15) + (size_t)8 * LANES * sizeof(float4);
+    bwd_long_vec_kernel<LANES, TPE><<<4 * kSmCount, 256, smem_long, st>>>(a);
+  } else {
+    bwd_long_scalar_kernel<<<4 * kSmCount, 256, sl, st>>>(a);
+  }
+}
+
+// radix engine: runs kernel, then the hot-row kernel.  Vector rows and dim 1: a warp per 32 sorted positions,
+// 8 warps per CTA; other dims: a thread per (sorted position, column).
+template <int LANES>
+static void launch_radix(const BwdArgs& a, cudaStream_t st) {
   const size_t smem = slot_smem_bytes(a.n_slots);
-  // one warp per 32 sorted positions, 8 warps per CTA
-  const unsigned grid = (unsigned)(a.main_ctas + a.or_chunks * a.n_slots);
-  if constexpr (LANES <= 8) {
+  const unsigned grid = (unsigned)ceil_div(a.n, 256);
+  if constexpr (LANES > 8) {
+    bwd_runs_vec_kernel<LANES><<<grid, 256, smem, st>>>(a);
+  } else if constexpr (LANES > 0) {
     const size_t smem_scan = ((smem + 15) & ~(size_t)15) + (size_t)8 * 32 * LANES * sizeof(float4);
     bwd_scan_vec_kernel<LANES><<<grid, 256, smem_scan, st>>>(a);
+  } else if (a.dim == 1) {
+    bwd_scan_d1_kernel<<<grid, 256, smem, st>>>(a);
   } else {
-    bwd_runs_vec_kernel<LANES><<<grid, 256, smem, st>>>(a);
+    bwd_runs_scalar_kernel<<<(unsigned)ceil_div(a.n * a.dim, 256), 256, smem, st>>>(a);
   }
-  constexpr int TPE = (LANES <= 8) ? 1 : LANES;
-  const size_t smem_long = ((smem + 15) & ~(size_t)15) + (size_t)8 * LANES * sizeof(float4);
-  bwd_long_vec_kernel<LANES, TPE><<<4 * kSmCount, 256, smem_long, st>>>(a);
+  launch_long<LANES>(a, st);
   count_launches(2);
 }
 
@@ -1662,14 +1654,7 @@ static void bk_launch_fused(BwdArgs a, const BwdWs& place, bool place_warp_mode,
   a.main_ctas = k.warp_ctas + k.med_ctas;
   bk_fused_kernel<LANES><<<k.warp_ctas + k.med_ctas + extra, bk::kThreads, smem, st>>>(a, k);
   bk_reduce_big_kernel<LANES><<<kSmCount, bk::kBigThreads, smem_big, st>>>(a, k);
-  const size_t sl = slot_smem_bytes(a.n_slots);
-  if constexpr (LANES > 0) {
-    constexpr int TPE = (LANES <= 8) ? 1 : LANES;
-    const size_t smem_long = ((sl + 15) & ~(size_t)15) + (size_t)8 * LANES * sizeof(float4);
-    bwd_long_vec_kernel<LANES, TPE><<<4 * kSmCount, 256, smem_long, st>>>(a);
-  } else {
-    bwd_long_scalar_kernel<<<4 * kSmCount, 256, sl, st>>>(a);
-  }
+  launch_long<LANES>(a, st);
   count_launches(3);
 }
 
@@ -1733,10 +1718,9 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
   BwdWs w = bwd_carve(ws, n_lookups_cap, dim);
   // number of live lookups: row_ptr[n_seg] when CSR (device side), else the capacity
   const int32_t* n_dev = row_ptr ? row_ptr + n_seg : nullptr;
-  // Two dedup engines.  Bucketed (bucket_bwd.cuh) is the product path; the global radix sort + scan is kept for
-  // the calls that also want the deduplicated gradient written out sorted by row (uniq_rows), and as the A/B
-  // reference (ER_K7=radix in the environment).
-  const bool bucketed = (uniq_rows == nullptr) && !k7_radix_forced();
+  // Two dedup engines.  Bucketed (bucket_bwd.cuh) updates tables; the global radix sort + scan serves the calls that
+  // also want the deduplicated gradient written out sorted by row (uniq_rows).
+  const bool bucketed = (uniq_rows == nullptr);
   // one-row slots (ER_BUCKET_ONE_ROW) bypass the dedup when lookup == segment (no CSR lookups in the call)
   const bool one_row = bucketed && seg_ids == nullptr;
   BwdWs src = w;
@@ -1744,11 +1728,9 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
     // the same lookups were placed / sorted by an earlier call on this stream (a table with the same row plan)
     if (sorted_ws_bytes < bwd_ws_bytes(n_lookups_cap, sorted_dim))
       return fail(ER_ERR_WORKSPACE, "er_embedding_bwd_reuse_sort: source workspace too small");
-    if (!bucketed && !k7_radix_forced())
+    if (!bucketed)
       return fail(ER_ERR_UNSUPPORTED, "er_embedding_bwd_reuse_sort: uniq_rows output needs the rows (er_embedding_bwd)");
     src = bwd_carve(const_cast<void*>(sorted_ws), n_lookups_cap, sorted_dim);
-    w.keys = src.keys;
-    w.vals = src.vals;
     cudaMemsetAsync(w.counters, 0, bk::zero_call_bytes(), st);
   } else if (bucketed) {
     bk_place(rows, n_lookups_cap, n_dev, n_rows, seg_ids, slots, n_slots, one_row, k7_warp_mode(dim), w, true, st);
@@ -1761,7 +1743,7 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
     return fail(ER_ERR_UNSUPPORTED, "er_embedding_bwd_reuse_sort: the placement was made for warp-sized buckets, "
                                     "rows of this dim need CTA-sized ones (presort with this dim instead)");
 
-  BwdArgs a;
+  BwdArgs a = {};
   a.table = table;
   a.state0 = state0;
   a.state1 = state1;
@@ -1796,7 +1778,6 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
   a.run_done = w.run_done;
   a.chunk_list = w.chunk_list;
   a.partials = w.partials;
-  a.main_ctas = (int)ceil_div(n_lookups_cap, 256);
   a.or_rows = rows;
   a.or_partials = w.one_row_partials;
   a.or_tickets = w.tickets;
@@ -1837,24 +1818,15 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
   }
   if (vec_dim && aligned) {
     switch (dim / 4) {
-      case 1: launch_vec<1>(a, st); break;
-      case 2: launch_vec<2>(a, st); break;
-      case 4: launch_vec<4>(a, st); break;
-      case 8: launch_vec<8>(a, st); break;
-      case 16: launch_vec<16>(a, st); break;
-      default: launch_vec<32>(a, st); break;
+      case 1: launch_radix<1>(a, st); break;
+      case 2: launch_radix<2>(a, st); break;
+      case 4: launch_radix<4>(a, st); break;
+      case 8: launch_radix<8>(a, st); break;
+      case 16: launch_radix<16>(a, st); break;
+      default: launch_radix<32>(a, st); break;
     }
   } else {
-    const size_t smem = slot_smem_bytes(n_slots);
-    if (dim == 1) {
-      a.main_ctas = (int)ceil_div(a.n, 256);
-      bwd_scan_d1_kernel<<<(unsigned)(a.main_ctas + a.or_chunks * a.n_slots), 256, smem, st>>>(a);
-    } else {
-      a.main_ctas = (int)ceil_div(a.n * dim, 256);
-      bwd_runs_scalar_kernel<<<(unsigned)(a.main_ctas + a.or_chunks * a.n_slots), 256, smem, st>>>(a);
-    }
-    bwd_long_scalar_kernel<<<4 * kSmCount, 256, smem, st>>>(a);
-    count_launches(2);
+    launch_radix<0>(a, st);
   }
   ER_CUDA_LAUNCH_CHECK();
   return ER_OK;
@@ -1888,11 +1860,8 @@ extern "C" int er_embedding_bwd_presort(const int64_t* rows, int64_t n_rows, con
     return fail(ER_ERR_WORKSPACE, "er_embedding_bwd_presort: workspace too small");
   BwdWs w = bwd_carve(ws, n_lookups_cap, dim);
   const int32_t* n_dev = row_ptr ? row_ptr + n_seg : nullptr;
-  if (k7_radix_forced())
-    rsort::sort_rows(rows, n_lookups_cap, n_dev, n_rows, w.keys, w.vals, w.sort_ws, w.counters, as_stream(stream));
-  else
-    bk_place(rows, n_lookups_cap, n_dev, n_rows, seg_ids, slots, n_slots, seg_ids == nullptr, k7_warp_mode(dim), w,
-             false, as_stream(stream));
+  bk_place(rows, n_lookups_cap, n_dev, n_rows, seg_ids, slots, n_slots, seg_ids == nullptr, k7_warp_mode(dim), w, false,
+           as_stream(stream));
   ER_CUDA_LAUNCH_CHECK();
   return ER_OK;
 }

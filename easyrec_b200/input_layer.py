@@ -464,7 +464,7 @@ class InputLayer(object):
     forked = False
     for idx, (m, rows, w, outs, seg_ids) in enumerate(self._pending):
       # arenas with the same row plan (DeepFM / Wide&Deep: the wide dim-1 and the deep tables) look up the
-      # same rows tensor: the second K7 reuses the first one's radix sort.
+      # same rows tensor: the second K7 reuses the first one's bucket placement.
       hit = sorted_by.get(id(rows))
       # (a placement made for warp-sized buckets serves only tables whose rows a warp can stage)
       src = (hit[0], hit[1]) if (hit is not None and hit[2] == m.arena.n_rows and
@@ -587,7 +587,7 @@ class InputLayer(object):
     return out
 
   def _presort(self):
-    """K7's radix sort needs only the looked-up rows: start it now on a side stream so it runs under the
+    """K7's bucket placement needs only the looked-up rows: start it now on a side stream so it runs under the
     dense forward/backward instead of after it (joined in backward_update; captured as a fork/join)."""
     self._presorted = {}
     if not (self.presort_enabled and not self.ep and torch.is_grad_enabled() and str(self.device).startswith('cuda')):

@@ -207,9 +207,14 @@ int er_embedding_fwd(const float* table, int64_t n_rows, int32_t dim,
  * bucket is sorted on (row, lookup) in shared memory: the deterministic
  * equivalent of TF's _deduplicate_indexed_slices), multiplied by
  * opt.grad_scale, and applied to the row and its optimizer state in the
- * same kernel.  Slots of mode ER_BUCKET_ONE_ROW take a weighted column sum
- * instead.  state0/state1: adagrad accumulator | adam m, v (same layout
- * and stride as table; unused ones NULL).
+ * same kernel.  Rows with many lookups are summed by a fixed chunked tree
+ * instead (deterministic, but not the sequential order): runs of more than
+ * 64 lookups when uniq_rows is given, otherwise runs of more than 48 in a
+ * bucket that a whole CTA sorts.  When uniq_rows is given and dim is 1 or a
+ * vector width up to 32, shorter runs are also summed by a fixed tree (a
+ * warp's shuffle scan).  Slots of mode ER_BUCKET_ONE_ROW take a weighted
+ * column sum instead.  state0/state1: adagrad accumulator | adam m, v (same
+ * layout and stride as table; unused ones NULL).
  * When uniq_rows/uniq_grads are non-NULL the deduplicated gradient is ALSO
  * written there (compact, sorted by row; *n_uniq receives the count); pass
  * table == NULL to only emit it. */

@@ -1,10 +1,9 @@
 """GPU parity of K7 on the bucketed dedup (bucket_bwd.cuh: hash the lookups into buckets by row, one warp sorts each
 bucket on (row, lookup) in registers, the run kernels sum and apply) against the CPU oracle, through the C ABI.
 
-Equal rows come out adjacent and in ascending lookup order, as from the radix sort, so the sums have the same fixed
-order as before: sequential for dim > 32, a fixed shuffle tree for dim <= 32 (last-ulp differences to the oracle's
-sequential order), chunked trees for hot rows (tolerance stated).  Covered: every dim class (vector 4..128, scalar 1
-and 6), CSR with weights and mean / sqrtn scaling, dropped lookups, duplicates of one row that overflow a warp's
+Equal rows come out adjacent and in ascending lookup order, as from the radix sort, so short runs are summed in the
+oracle's sequential order and hot rows by fixed chunked trees (tolerance stated).  Covered: every dim class (vector
+4..128, scalar 1 and 6), CSR with weights and mean / sqrtn scaling, dropped lookups, duplicates of one row that overflow a warp's
 128 pairs (CTA sort), a CTA's 16384 pairs (global-memory radix fallback), one-row slots (ER_BUCKET_ONE_ROW), the
 presort + reuse split, clustered rows (identity ids), device-side lookup counts, and agreement with the radix engine
 (uniq_rows output) at the C2 size.
@@ -95,7 +94,7 @@ def _check(got, want, long_rows=()):
   cold = np.ones(want[0].shape[0], bool)
   cold[list(long_rows)] = False
   for g, w_ in zip(got, want):
-    # short runs: the oracle's order, or the fixed shuffle tree (dim <= 32): last-ulp differences
+    # short runs, summed in the oracle's order
     np.testing.assert_allclose(g[cold], w_[cold], rtol=2e-6, atol=2e-6)
     if long_rows:   # fixed-tree sums of hundreds..tens of thousands of N(0,1) gradients
       np.testing.assert_allclose(g[~cold], w_[~cold], rtol=2e-4, atol=2e-4)
