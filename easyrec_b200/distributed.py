@@ -8,8 +8,6 @@ every rank then runs the same deterministic dedup + fused row update over the gl
 replicas stay bit-identical without a broadcast.  Dense gradients: one flat all-reduce
 (`hvd.allreduce(g, Average)`, compat/optimizers.py:289-292).
 """
-import os
-
 import numpy as np
 import torch
 import torch.distributed as dist
@@ -114,12 +112,13 @@ class DataParallel(object):
     self._rows_owner = {}
     self._pre = {}
     self._side = None
-    self.prephase = os.environ.get('ER_DP_PREPHASE', '1') == '1' and str(getattr(input_layer, 'device', 'cpu')).startswith('cuda')
+    # the early exchange runs on a side stream; CPU runs and the calls it does not cover take the late one
+    self.prephase = str(getattr(input_layer, 'device', 'cpu')).startswith('cuda')
 
   def pre_exchange(self, features):
-    """Ahead of the step (eager, outside CUDA-graph capture): K1 on this rank's batch, all-gather of the rows
-    and per-lookup weights, and the global dedup sort started on a side stream - it needs no gradient, so
-    it runs under the dense forward/backward (with N ranks it is N times the single-GPU sort)."""
+    """At the head of the step: K1 on this rank's batch, all-gather of the rows and per-lookup weights, and the
+    global dedup sort started on a side stream - it needs no gradient, so it runs under the dense forward/backward
+    (with N ranks it is N times the single-GPU sort)."""
     if not self.prephase:
       return
     il = self.input_layer
@@ -222,8 +221,8 @@ class DataParallel(object):
       dist.all_gather_into_tensor(g.grads[i], grad.contiguous())
 
   def exchange(self, pending):
-    """The collectives of one step (eager NCCL calls, kept OUTSIDE CUDA-graph capture): dense flat
-    all-reduce + all-gather of every arena's K7 inputs."""
+    """The collectives of one step after the backward: dense flat all-reduce + all-gather of every arena's K7
+    inputs."""
     self.sync_dense_grads()
     if not self.sparse:
       return
@@ -232,16 +231,13 @@ class DataParallel(object):
       self.gather_sparse(call, rows, w, outs, seg_ids)
 
   def join_presort(self):
-    """main stream waits for the early global sorts (call before apply_sparse / its graph replay)."""
+    """main stream waits for the early global sorts (call before apply_sparse)."""
     if self._pre and self._side is not None:
       torch.cuda.current_stream().wait_stream(self._side)
 
   def apply_sparse(self, pending, opt):
     """The same fused dedup + row update on every rank over the gathered global batch; gradients
     are scaled by 1/world (mean over replicas).  No collectives: CUDA-graph capturable."""
-    if not self.sparse:
-      self.input_layer.backward_update()   # sharded tables: all-to-all of the gradients + K7 on the owners
-      return
     # mean over replicas: a caller that keeps the step scalars in device memory (InputLayer.hyper) has folded
     # 1/world into them (replica_grad_scale); a plain er_opt_t is scaled here
     struct_scaled = not opt.hyper_dev
@@ -264,11 +260,3 @@ class DataParallel(object):
       E.adam_dense_decay(a, owner.rows if not g.one_row else torch.cat([owner.rows, g.one_row_rows]), opt)
     if struct_scaled:
       opt.grad_scale = opt.grad_scale * self.world
-
-  def sparse_backward_update(self, opt):
-    il = self.input_layer
-    self._rows_owner = {}
-    for call, rows, w, outs, seg_ids in il._pending:
-      self.gather_sparse(call, rows, w, outs, seg_ids)
-    self.apply_sparse(il._pending, opt)
-    il._pending = []

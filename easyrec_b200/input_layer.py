@@ -560,9 +560,9 @@ class InputLayer(object):
     return buf
 
   def precompute_rows(self, features):
-    """K1 (index hashing / bucketing) of the single-valued slots ahead of the step, outside any CUDA-graph
-    capture: data-parallel training all-gathers the rows and starts the global dedup sort while the dense
-    forward/backward runs.  Returns [(arena dim, ArenaCall, rows, weights)]; the next lookup() reuses them."""
+    """K1 (index hashing / bucketing) of the single-valued slots at the head of the step, ahead of the lookup:
+    data-parallel training all-gathers the rows and starts the global dedup sort while the dense forward/backward
+    runs.  Returns [(arena dim, ArenaCall, rows, weights)]; the next lookup() reuses them."""
     dense = features.get('dense_fea')
     dense_norm = self.normalize_dense(dense) if dense is not None else None
     out = []

@@ -5,16 +5,10 @@
 Shard rule (bit-exact with the reference): owner = row mod N, local row = row div N, each worker holds
 (V + N - 1) // N rows of every table (feature_column.py:296,317,461-463); produced by er_bucketize.
 
-Two implementations live here:
-
-* `ShardedLookup` / `ShardedExchange` - the product path, what `InputLayer` runs for sharded arenas: distinct ids per
-  owner in FIXED-capacity blocks (K8 er_shard_group), equal-split all-to-alls, nothing read back on the host, the whole
-  exchange captured in the step's CUDA graph; arenas of one row plan share ids and one packed row exchange; the id half
-  can be prefetched a step ahead.
-* `ShardedArena` - round 1's stand-alone form with the reference's own data flow (sort by owner, counts exchanged and
-  read on the host like hvd.alltoall, per-lookup gradient rows): kept because it is pinned, lookup by lookup, to the
-  reference's `embedding_parallel_lookup` run (tests/golden/reference_lookup.json, tests/test_sharded_gloo.py,
-  tests/test_gpu_sharded.py).  Not CUDA-graph captured; single-valued slots only.
+`ShardedLookup` / `ShardedExchange` are what `InputLayer` runs for sharded arenas: distinct ids per owner in
+FIXED-capacity blocks (K8 er_shard_group), equal-split all-to-alls, nothing read back on the host, the whole exchange
+captured in the step's CUDA graph; arenas of one row plan share ids and one packed row exchange; the id half can be
+prefetched a step ahead.
 """
 import os
 
@@ -25,109 +19,6 @@ import torch.distributed as dist
 from easyrec_b200 import _lib
 from easyrec_b200 import embedding as E
 from easyrec_b200 import kernels as K
-
-
-class ShardedArena(object):
-
-  def __init__(self, dim, tables, slots, batch_size, device, world, rank, opt_kind=_lib.OPT_ADAGRAD,
-               generator=None, init_full=None):
-    """tables: list of (name, n_rows_global); slots: list of E.Slot over those tables (single-valued).
-    init_full: optional full [sum V, dim] tensor (same on every rank) from which the local shard is cut
-    -- used by the tests to compare against an unsharded run."""
-    self.dim, self.world, self.rank, self.device = dim, world, rank, device
-    self.batch_size = batch_size
-    self.arena = E.Arena(dim, device, shard_n=world, shard_rank=rank)
-    self.global_offsets = {}
-    g = 0
-    for name, v in tables:
-      self.arena.add_table(name, v)
-      self.global_offsets[name] = (g, v)
-      g += v
-    if init_full is not None:
-      def init_fn(w):
-        for name, v in tables:
-          off, local, _ = self.arena.tables[name]
-          g0, _ = self.global_offsets[name]
-          shard = init_full[g0:g0 + v][rank::world]
-          w[off:off + shard.shape[0]].copy_(shard)
-          if shard.shape[0] < local:
-            w[off + shard.shape[0]:off + local].zero_()
-      self.arena.materialize(opt_kind, init_fn=init_fn)
-    else:
-      self.arena.materialize(opt_kind, generator=generator)
-    F = len(slots)
-    self.n_slots = F
-    self.call = E.ArenaCall(self.arena, slots, batch_size, [F * dim], single_valued=True)
-    self.L = self.call.n_seg
-    # plan that pools the RECEIVED rows (a [L, dim] "table" indexed by sorted position)
-    recs = []
-    for r in self.call.slots_np:
-      recs.append(dict(num_buckets=self.L, row_offset=0, seg_begin=int(r['seg_begin']), n_seg=int(r['n_seg']),
-                       bucket_mode=_lib.BUCKET_NONE, combiner=int(r['combiner']), out_buf=0,
-                       out_stride=int(r['out_stride']), out_col=int(r['out_col']), shard_n=1))
-    self.pool_slots = K.slots_to_device(K.make_slots(recs), device)
-    # single-slot plan for owner-side gather / update over a variable number of received rows
-    self.cap = max(4 * self.L, 1024)
-    own = [dict(num_buckets=self.arena.n_rows, row_offset=0, seg_begin=0, n_seg=self.cap, bucket_mode=_lib.BUCKET_NONE,
-                combiner=_lib.COMBINER_SUM, out_buf=0, out_stride=dim, out_col=0, shard_n=1)]
-    self.owner_slots = K.slots_to_device(K.make_slots(own), device)
-    self.owner_ws = K.bwd_workspace(self.cap, device, dim)
-    self._ctx = None
-
-  def lookup(self, ids, weights=None):
-    """ids int64 [F*B] feature-major.  Returns the pooled group matrix [B, F*dim] (autograd leaf)."""
-    N, dev, D = self.world, self.device, self.dim
-    call = self.call
-    owner = torch.empty(self.L, dtype=torch.int32, device=dev)
-    rows_local = K.bucketize(ids, call.slots_dev, call.n_slots, call.n_seg, owner=owner)
-    # group the lookups by owner (dropped lookups: owner -1 -> sentinel key N, sorted last, never sent)
-    keys, perm = K.sort_rows(torch.where(owner < 0, torch.full_like(owner, -1), owner).to(torch.int64), N)
-    perm = perm.to(torch.int64)
-    send_counts = torch.bincount(owner[owner >= 0].to(torch.int64), minlength=N)
-    recv_counts = torch.empty_like(send_counts)
-    dist.all_to_all_single(recv_counts, send_counts)
-    sc, rc = send_counts.tolist(), recv_counts.tolist()   # host sync, as hvd.alltoall does
-    n_send, n_recv = sum(sc), sum(rc)
-    assert n_recv <= self.cap, 'received %d rows > capacity %d' % (n_recv, self.cap)
-    send_rows = rows_local[perm[:n_send]].contiguous()
-    recv_rows = torch.empty(n_recv, dtype=torch.int64, device=dev)
-    dist.all_to_all_single(recv_rows, send_rows, rc, sc)
-    # owner side: gather the requested rows of the local shard
-    send_emb = torch.empty(max(n_recv, 1), D, dtype=torch.float32, device=dev)
-    if n_recv:
-      K.embedding_fwd(self.arena.weight, D, recv_rows, self.owner_slots, 1, n_recv, [send_emb])
-    recv_emb = torch.empty(max(n_send, 1), D, dtype=torch.float32, device=dev)
-    dist.all_to_all_single(recv_emb[:n_send], send_emb[:n_recv], sc, rc)
-    # requester side: position of every lookup inside recv_emb, then pool into the group layout
-    pos = torch.full((self.L,), -1, dtype=torch.int64, device=dev)
-    pos[perm[:n_send]] = torch.arange(n_send, device=dev)
-    out = torch.empty(self.batch_size, call.out_strides[0], dtype=torch.float32, device=dev)
-    K.embedding_fwd(recv_emb, D, pos, self.pool_slots, self.n_slots, self.L, [out], weights=weights)
-    out.requires_grad_(True)
-    self._ctx = (perm, n_send, sc, rc, recv_rows, weights, out)
-    return out
-
-  def backward_update(self, opt):
-    """Send each lookup's gradient row to its owner; owners dedup + apply with grad_scale / N."""
-    perm, n_send, sc, rc, recv_rows, weights, out = self._ctx
-    N, D, B, F = self.world, self.dim, self.batch_size, self.n_slots
-    g = out.grad[:, :F * D].reshape(B, F, D).permute(1, 0, 2).reshape(self.L, D)  # per-lookup rows
-    if weights is not None:
-      g = g * weights[:, None]
-    send_g = g[perm[:n_send]].contiguous()
-    n_recv = sum(rc)
-    recv_g = torch.empty(max(n_recv, 1), D, dtype=torch.float32, device=self.device)
-    dist.all_to_all_single(recv_g[:n_recv], send_g, rc, sc)
-    if n_recv:
-      struct_scaled = not opt.hyper_dev   # a device-resident grad_scale already carries the 1/N
-      if struct_scaled:
-        opt.grad_scale = opt.grad_scale / N
-      K.embedding_bwd(self.arena.weight, self.arena.state0, self.arena.state1, D, recv_rows, self.owner_slots, 1,
-                      n_recv, [recv_g], opt, self.owner_ws, n_rows=self.arena.n_rows)
-      if struct_scaled:
-        opt.grad_scale = opt.grad_scale * N
-    E.adam_dense_decay(self.arena, recv_rows if n_recv else None, opt)
-    self._ctx = None
 
 
 class ShardedExchange(object):

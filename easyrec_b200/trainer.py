@@ -9,7 +9,6 @@ batch-8192 step: SURVEY.md section 8d); the learning rate lives in device memory
 does not need a re-capture.
 """
 import ctypes
-import os
 
 import numpy as np
 import torch
@@ -220,7 +219,6 @@ class Trainer(object):
     self._static_next = None
     self._warm_stream = None
     self._graph = None
-    self._graph2 = None
     self._step_pending = []
     self._static = None
     self._loss = None
@@ -232,8 +230,8 @@ class Trainer(object):
     if self.dense_lr_fn is not None:
       self.dense_opt.hyper.set(self.dense_lr_fn(self.step), self.step)
 
-  # The step is three segments; only the middle one talks to other ranks, so with world > 1 the
-  # CUDA graph is captured as two graphs around eager NCCL calls.
+  # The step is three segments; only the middle one talks to other ranks (world > 1).  A CUDA graph
+  # captures all three, the collectives included.
   def _segment_compute(self, features, labels, next_features=None):
     """lookup -> model -> loss -> backward -> dense grads into the flat buffer."""
     self.dense_opt.zero_grad()
@@ -255,11 +253,12 @@ class Trainer(object):
 
   def _segment_exchange(self):
     if self.dp is not None:
-      if not self.dp.sparse and self._ep_side is not None:
-        # row-sharded tables: their backward (gradient sums, all-to-all to the owners, owner-side row update) is a
-        # parallel branch beside the dense all-reduce + dense optimizer; joined at the end of _segment_update
-        self._ep_side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(self._ep_side):
+      if not self.dp.sparse:
+        # row-sharded tables: their backward (gradient sums, all-to-all to the owners, owner-side row update); on CUDA
+        # a parallel branch beside the dense all-reduce + dense optimizer, joined in _segment_update
+        if self._ep_side is not None:
+          self._ep_side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(self._ep_side):   # (no side stream: a no-op)
           self.input_layer.backward_update()
       self.dp.exchange(self._step_pending)   # flat all-reduce + all-gather of K7 inputs
       self.dp.join_presort()
@@ -294,16 +293,11 @@ class Trainer(object):
 
   def _segment_update(self, loss):
     if self.clip_norm:
-      ep = self.dp is not None and not self.dp.sparse
-      if ep:
-        if self._ep_side is not None:
-          torch.cuda.current_stream().wait_stream(self._ep_side)   # the gradient exchange of _segment_exchange
-        else:
-          self.input_layer.backward_update()   # (host build) gradient sums + all-to-all; the owners hold their update
+      if self._ep_side is not None:
+        torch.cuda.current_stream().wait_stream(self._ep_side)   # the gradient exchange of _segment_exchange
       self._clip_by_global_norm()
-      if ep:
+      if self.dp is not None and not self.dp.sparse:
         self.input_layer.ep_apply_held()       # owner-side K7 with the clipped, 1/N-scaled gradient scale
-        self.input_layer._pending = []
         self.dense_opt.apply(l2_folded=True, grad_scale=1.0)
       elif self.dp is not None:
         # the gathered K7 reads the clip factor from the device-resident gradient scale (x 1/N, replica_grad_scale);
@@ -315,25 +309,20 @@ class Trainer(object):
         self.input_layer.backward_update()
         self.dense_opt.apply(l2_folded=True)
       return loss + self.dense_opt.reg_loss[0]
-    if self.dp is not None and not self.dp.sparse and self._ep_side is not None:
-      self.input_layer._pending = []
-    elif self.dp is not None:
+    if self.dp is None:
+      self.input_layer.backward_update()   # K7: dedup + fused row update, on this thread/stream
+    elif self.dp.sparse:
       self.dp.apply_sparse(self._step_pending, self.input_layer.opt_holder['opt'])
       self.input_layer._pending = []
-    else:
-      self.input_layer.backward_update()   # K7: dedup + fused row update, on this thread/stream
     self.dense_opt.apply()                 # one launch: l2 + adagrad/adam over the flat buffer
-    if self.dp is not None and not self.dp.sparse and self._ep_side is not None:
-      torch.cuda.current_stream().wait_stream(self._ep_side)
+    if self._ep_side is not None:
+      torch.cuda.current_stream().wait_stream(self._ep_side)   # the row-sharded backward of _segment_exchange
     # reported loss = data loss + embedding regularisation (autograd) + dense l2 (from the apply)
     return loss + self.dense_opt.reg_loss[0]
 
-  def _segment_pre(self, features):
-    if self.dp is not None:
-      self.dp.pre_exchange(features)   # eager: K1 + all-gather of rows + global dedup sort on a side stream
-
   def _step_body(self, features, labels, next_features=None):
-    self._segment_pre(features)
+    if self.dp is not None:
+      self.dp.pre_exchange(features)   # K1 + all-gather of rows + global dedup sort on a side stream
     loss, probs = self._segment_compute(features, labels, next_features)
     self._segment_exchange()
     out = self._segment_update(loss), probs
@@ -385,16 +374,11 @@ class Trainer(object):
         self.input_layer.prefetch_exchange(self._static_feats)
         self.input_layer.join_prefetch()
       self._stale_next = next_features is None
-    if self._graph2 is not None:
-      self._segment_pre(self._static_feats)
     self._graph.replay()
     if self._prefetch_mode:
       # the replay promoted and prefetched on its own; an EAGER lookup after it (evaluate / predict) must not take
       # the graph's prefetched ids for its own
       self.input_layer.drop_prefetch()
-    if self._graph2 is not None:   # world > 1: collectives between the two captured segments
-      self._segment_exchange()
-      self._graph2.replay()
     self.step += 1
     return self._loss, self._probs
 
@@ -417,22 +401,9 @@ class Trainer(object):
     n0 = _lib.load().er_launch_count()
     # Data parallel: the collectives (NCCL on the capture stream) are captured with the rest of the step - one
     # graph per step.  capture_error_mode 'thread_local': NCCL's watchdog thread polls CUDA events while this
-    # thread captures, which the default global mode treats as a capture violation.  ER_DP_ONE_GRAPH=0 keeps the
-    # collectives eager between two captured segments.
-    one_graph = self.dp is None or os.environ.get('ER_DP_ONE_GRAPH', '1') == '1'
-    if one_graph:
-      kw = {} if self.dp is None else {'capture_error_mode': 'thread_local'}
-      with torch.cuda.graph(self._graph, **kw):
-        self._loss, self._probs = self._step_body(feats, self._static['__labels'], self._static_next)
-    else:
-      self._segment_pre(feats)   # eager, before the capture: the captured lookup reuses these rows
-      with torch.cuda.graph(self._graph):
-        loss, self._probs = self._segment_compute(feats, self._static['__labels'])
-      # eager and on stale buffers (graph 1 has not run yet): it only fixes which gathered buffers the update
-      # segment reads - every buffer it touches is rewritten by the first replay before it is used
-      self._segment_exchange()
-      self._graph2 = torch.cuda.CUDAGraph()
-      with torch.cuda.graph(self._graph2, pool=self._graph.pool()):
-        self._loss = self._segment_update(loss)
-    # kernels of liber_b200.so inside one replay of the graph(s)
+    # thread captures, which the default global mode treats as a capture violation.
+    kw = {} if self.dp is None else {'capture_error_mode': 'thread_local'}
+    with torch.cuda.graph(self._graph, **kw):
+      self._loss, self._probs = self._step_body(feats, self._static['__labels'], self._static_next)
+    # kernels of liber_b200.so inside one replay of the graph
     self.launches_per_step = int(_lib.load().er_launch_count() - n0)

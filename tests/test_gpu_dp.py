@@ -3,9 +3,9 @@
 Checks: (1) replicas stay BIT-identical (tables, optimizer state, dense parameters) - K7 and the dense path
 are deterministic and every rank applies the same gathered update; (2) the early exchange (K1 + all-gather
 of rows + global dedup sort on a side stream before the step) gives exactly the same model as the plain
-exchange after the backward pass; (3) CUDA-graph replay - collectives eager between two captured segments, and
-captured inside ONE graph per step (NCCL on the capture stream) - trains exactly the same model as the eager run
-(2 eager steps, capture, replays: every batch applied once).  Skipped on boxes with fewer than 2 GPUs."""
+exchange after the backward pass; (3) CUDA-graph replay - the collectives captured inside ONE graph per step (NCCL
+on the capture stream) - trains exactly the same model as the eager run (2 eager steps, capture, replays: every batch
+applied once).  Skipped on boxes with fewer than 2 GPUs."""
 import os
 import socket
 
@@ -28,10 +28,10 @@ def _train(rank, dev, prephase, graph, steps=4):
   import torch.distributed as dist
   from easyrec_b200 import workloads
   from easyrec_b200.trainer import Trainer
-  os.environ['ER_DP_PREPHASE'] = '1' if prephase else '0'
   B, V = 512, 50021
   il, model = workloads.build_deepfm_criteo(B, V, dev, dnn=(64, 32), final=(32, 16), seed=11)
   tr = Trainer(model, il, 'adagrad', lr=0.05, use_cuda_graph=graph, world_size=WORLD)
+  tr.dp.prephase = prephase   # False: the rows are all-gathered with the gradients after the backward
   for step in range(steps):
     ids, dense, labels = workloads.criteo_batch(B, 100 + 10 * step + rank)
     feats = {'sparse_fea': torch.from_numpy(ids).to(dev), 'dense_fea': torch.from_numpy(dense).to(dev)}
@@ -50,9 +50,7 @@ def _worker(rank, port, ret):
   dist.init_process_group('nccl', rank=rank, world_size=WORLD, device_id=torch.device(dev))
   torch.backends.cuda.matmul.allow_tf32 = False
   results = {}
-  for name, (pre, graph, one) in {'plain': (False, False, '1'), 'early': (True, False, '1'),
-                                  'graph_two_segments': (True, True, '0'), 'graph_one': (True, True, '1')}.items():
-    os.environ['ER_DP_ONE_GRAPH'] = one
+  for name, (pre, graph) in {'plain': (False, False), 'early': (True, False), 'graph_one': (True, True)}.items():
     loss, state = _train(rank, dev, pre, graph, steps=6)
     assert loss == loss and abs(loss) < 10
     for t in state:   # replicas identical: max over ranks of |mine - rank0's| must be exactly 0
@@ -60,7 +58,7 @@ def _worker(rank, port, ret):
       dist.broadcast(ref, src=0)
       assert torch.equal(t, ref), '%s: replicas diverged' % name
     results[name] = state
-  for other in ('early', 'graph_two_segments', 'graph_one'):
+  for other in ('early', 'graph_one'):
     for a, b in zip(results['plain'], results[other]):
       assert torch.equal(a, b), '%s: a different model than the plain eager exchange' % other
   ret[rank] = True

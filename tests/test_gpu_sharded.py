@@ -1,5 +1,5 @@
-"""2 GPUs: the row-sharded (EmbeddingParallel) arena with NCCL all-to-all vs the CPU oracle run on the
-unsharded table and the concatenated global batch.  Skipped on boxes with fewer than 2 GPUs.
+"""2 GPUs: the row-sharded (EmbeddingParallel) lookup, sharded.ShardedLookup with NCCL all-to-all, vs the CPU oracle
+run on the unsharded table and the concatenated global batch.  Skipped on boxes with fewer than 2 GPUs.
 
 Checks: owner/local-row rule (bit exact, via the pooled values), forward pooled outputs (exact: each
 output is a copy/sum of table rows in lookup order), and the post-step shards after the gradient
@@ -31,7 +31,7 @@ def _worker(rank, port, ret):
   dev = 'cuda:%d' % rank
   dist.init_process_group('nccl', rank=rank, world_size=WORLD, device_id=torch.device(dev))
   from easyrec_b200 import _lib, embedding as E, kernels as K
-  from easyrec_b200.sharded import ShardedArena
+  from easyrec_b200.sharded import ShardedLookup
   from oracle import oracle as O
   B, D = 512, 16
   tables = [('t0', 10007), ('t1', 5003)]
@@ -39,22 +39,38 @@ def _worker(rank, port, ret):
   slots = [E.Slot('s%d' % i, t, m, nb) for i, (m, nb, t) in enumerate(modes)]
   F = len(slots)
   full = torch.from_numpy(np.random.default_rng(7).normal(0, 0.01, (10007 + 5003, D)).astype(np.float32))
-  sa = ShardedArena(D, tables, slots, B, dev, WORLD, rank, init_full=full.to(dev))
+  g0 = {'t0': 0, 't1': 10007}
+  arena = E.Arena(D, dev, shard_n=WORLD, shard_rank=rank)
+  for name, v in tables:
+    arena.add_table(name, v)
+
+  def init_fn(w):
+    w.zero_()
+    for name, v in tables:
+      off = arena.tables[name][0]
+      shard = full[g0[name]:g0[name] + v][rank::WORLD]
+      w[off:off + shard.shape[0]].copy_(shard)
+  arena.materialize(_lib.OPT_ADAGRAD, init_fn=init_fn)
+  call = E.ArenaCall(arena, slots, B, [F * D], single_valued=True)
+  sl = ShardedLookup(call, WORLD, rank)
   rng = np.random.default_rng(100 + rank)
   ids = (rng.zipf(1.2, F * B) % 50000).astype(np.int64)
   ids[rng.integers(0, F * B, 20)] = -5  # negative ids are valid for hash / floored mod
-  out = sa.lookup(torch.from_numpy(ids).to(dev))
+  outs = call.alloc_outputs()
+  sl.forward(torch.from_numpy(ids).to(dev), None, outs)
+  sl.check()                            # no lookup lost to a full per-peer block
+  out = outs[0]
   # ---- oracle: unsharded rows and pooled outputs ----
   mode_l = np.repeat([m for m, _, _ in modes], B)
   nb_l = np.repeat([nb for _, nb, _ in modes], B)
-  off_l = np.repeat([0 if t == 't0' else 10007 for _, _, t in modes], B)
+  off_l = np.repeat([g0[t] for _, _, t in modes], B)
   g_rows, _ = O.bucketize(ids, mode_l, nb_l, off_l)
   want = full.numpy()[g_rows].reshape(F, B, D).transpose(1, 0, 2).reshape(B, F * D)
-  assert np.array_equal(out.detach().cpu().numpy(), want), 'sharded forward differs'
+  assert np.array_equal(out.cpu().numpy(), want), 'sharded forward differs'
   # ---- backward: all ranks' gradients meet on the owners ----
   gout = rng.normal(0, 0.1, (B, F * D)).astype(np.float32)
   out.grad = torch.from_numpy(gout).to(dev)
-  sa.backward_update(K.make_opt(_lib.OPT_ADAGRAD, 0.05))
+  sl.backward_update(outs, K.make_opt(_lib.OPT_ADAGRAD, 0.05))
   torch.cuda.synchronize()
   # gather everyone's (rows, grads) on the host and run the oracle on the global batch
   all_rows = [None] * WORLD
@@ -66,12 +82,11 @@ def _worker(rank, port, ret):
   O.embedding_bwd(t, acc, None, np.concatenate(all_rows), None, np.concatenate(all_g), O.OPT_ADAGRAD, 0.05,
                   grad_scale=1.0 / WORLD)
   for name, v in tables:
-    off, local, _ = sa.arena.tables[name]
-    g0 = 0 if name == 't0' else 10007
-    want_shard = t[g0:g0 + v][rank::WORLD]
-    got = sa.arena.weight[off:off + want_shard.shape[0]].cpu().numpy()
+    off = arena.tables[name][0]
+    want_shard = t[g0[name]:g0[name] + v][rank::WORLD]
+    got = arena.weight[off:off + want_shard.shape[0]].cpu().numpy()
     np.testing.assert_allclose(got, want_shard, rtol=0, atol=1e-6)
-    assert (got != full.numpy()[g0:g0 + v][rank::WORLD]).any()
+    assert (got != full.numpy()[g0[name]:g0[name] + v][rank::WORLD]).any()
   ret[rank] = True
   dist.destroy_process_group()
 

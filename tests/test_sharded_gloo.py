@@ -1,19 +1,23 @@
-"""CPU, world_size 2 and 8 over gloo: the HOST logic of the row-sharded arena (easyrec_b200/sharded.py) -
-owner grouping, the three all-to-all exchanges with data-dependent split sizes, the position map that pools
-the received rows, the gradient exchange and the 1/N scaling (compat/optimizers.py:315-316).
+"""CPU, world_size 2 and 8 over gloo: the HOST logic of the row-sharded lookup (easyrec_b200/sharded.py
+ShardedLookup) - owner grouping into fixed-capacity per-peer blocks, the id / row / gradient all-to-alls, the position
+map that pools the received rows, the requester-side duplicate sums and the owner-side 1/N gradient scale
+(compat/optimizers.py:315-316).
 
-The CUDA kernels cannot run here, so `sharded.K` is replaced by a double with the same call signatures whose
-bodies are the CPU oracle (bucketize / pooling / dedup + Adagrad) - the kernels themselves are compared with that
-oracle on the GPU (tests/test_gpu_sparse.py, tests/test_gpu_sharded.py on 2 GPUs).  Every rank checks its pooled
-output and its updated shard against the oracle run on the UNSHARDED table and the concatenated global batch."""
+The CUDA kernels cannot run here, so they are replaced by the oracle-backed doubles of tests/host_doubles.py - the
+kernels themselves are compared with that oracle on the GPU (tests/test_gpu_sparse.py, tests/test_gpu_sharded.py on
+2 GPUs).  Every rank checks its pooled output and its updated shard against the oracle run on the UNSHARDED table and
+the concatenated global batch."""
 import os
 import socket
+import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
+
+HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def _free_port():
@@ -24,77 +28,52 @@ def _free_port():
   return p
 
 
-class OracleKernels(object):
-  """stand-in for easyrec_b200.kernels inside sharded.py (CPU tensors)."""
-
-  def __init__(self):
-    from easyrec_b200 import kernels as K
-    from oracle import oracle as O
-    self.K, self.O = K, O
-    self.make_slots, self.slots_to_device, self.bwd_workspace = K.make_slots, K.slots_to_device, K.bwd_workspace
-
-  def _slots(self, slots_dev):
-    return np.frombuffer(slots_dev.numpy().tobytes(), dtype=self.K.SLOT_DTYPE)
-
-  def bucketize(self, ids, slots_dev, n_slots, n_seg, owner=None):
-    sl = self._slots(slots_dev)
-    per = lambda f: np.concatenate([np.full(int(s['n_seg']), s[f]) for s in sl])   # noqa: E731
-    rows, own = self.O.bucketize(ids.numpy(), per('bucket_mode'), per('num_buckets'), per('row_offset'), shard_n=per('shard_n'))
-    owner.copy_(torch.from_numpy(own))
-    return torch.from_numpy(rows)
-
-  def sort_rows(self, keys, max_row):
-    k = keys.numpy()
-    k = np.where(k < 0, max_row, k)
-    perm = np.argsort(k, kind='stable')
-    return torch.from_numpy(k[perm]), torch.from_numpy(perm.astype(np.int64))
-
-  def embedding_fwd(self, table, dim, rows, slots_dev, n_slots, n_seg, outs, weights=None):
-    t, r = table.numpy(), rows.numpy()
-    left = n_seg
-    for s in self._slots(slots_dev):
-      out = outs[int(s['out_buf'])]
-      for k in range(min(int(s['n_seg']), left)):
-        l = int(s['seg_begin']) + k
-        v = t[r[l]] * (float(weights[l]) if weights is not None else 1.0) if r[l] >= 0 else np.zeros(dim, np.float32)
-        out.view(-1)[k * int(s['out_stride']) + int(s['out_col']):][:dim] = torch.from_numpy(np.asarray(v, np.float32))
-      left -= int(s['n_seg'])
-
-  def embedding_bwd(self, weight, s0, s1, dim, rows, slots_dev, n_slots, n_seg, grads, opt, ws, n_rows=None):
-    w, a = np.ascontiguousarray(weight.numpy()), np.ascontiguousarray(s0.numpy())
-    self.O.embedding_bwd(w, a, None, rows.numpy()[:n_seg], None, grads[0].numpy()[:n_seg], self.O.OPT_ADAGRAD, opt.lr,
-                         grad_scale=opt.grad_scale)
-    weight.copy_(torch.from_numpy(w))
-    s0.copy_(torch.from_numpy(a))
-
-
 def _worker(rank, port, ret, world):
   os.environ['MASTER_ADDR'] = '127.0.0.1'
   os.environ['MASTER_PORT'] = str(port)
   dist.init_process_group('gloo', rank=rank, world_size=world)
-  from easyrec_b200 import _lib, embedding as E, kernels as K, sharded
+  sys.path.insert(0, HERE)
+  import host_doubles
+  host_doubles.install_sparse(setattr)
+  from easyrec_b200 import _lib, embedding as E, kernels as K
+  from easyrec_b200.sharded import ShardedLookup
   from oracle import oracle as O
-  sharded.K = OracleKernels()
   B, D = 24, 4
   tables = [('t0', 101), ('t1', 37)]                      # odd sizes: the last shards carry padding rows
   modes = [(_lib.BUCKET_FARM_DECIMAL, 101, 't0'), (_lib.BUCKET_MOD, 37, 't1'), (_lib.BUCKET_FARM_DECIMAL, 101, 't0')]
   slots = [E.Slot('s%d' % i, t, m, nb) for i, (m, nb, t) in enumerate(modes)]
   F = len(slots)
   full = torch.from_numpy(np.random.default_rng(7).normal(0, 0.1, (101 + 37, D)).astype(np.float32))
-  sa = sharded.ShardedArena(D, tables, slots, B, 'cpu', world, rank, init_full=full)
+  g0 = {'t0': 0, 't1': 101}
+  arena = E.Arena(D, 'cpu', shard_n=world, shard_rank=rank)
+  for name, v in tables:
+    arena.add_table(name, v)
+
+  def init_fn(w):
+    w.zero_()
+    for name, v in tables:
+      off = arena.tables[name][0]
+      shard = full[g0[name]:g0[name] + v][rank::world]
+      w[off:off + shard.shape[0]].copy_(shard)
+  arena.materialize(_lib.OPT_ADAGRAD, init_fn=init_fn)
+  call = E.ArenaCall(arena, slots, B, [F * D], single_valued=True)
+  sl = ShardedLookup(call, world, rank)
   rng = np.random.default_rng(100 + rank)
   ids = (rng.zipf(1.3, F * B) % 5000).astype(np.int64)
   ids[rng.integers(0, F * B, 5)] = -5
-  out = sa.lookup(torch.from_numpy(ids))
+  outs = call.alloc_outputs()
+  sl.forward(torch.from_numpy(ids), None, outs)
+  sl.check()                                              # no lookup lost to a full per-peer block
+  out = outs[0]
   mode_l = np.repeat([m for m, _, _ in modes], B)
   nb_l = np.repeat([nb for _, nb, _ in modes], B)
-  off_l = np.repeat([0 if t == 't0' else 101 for _, _, t in modes], B)
+  off_l = np.repeat([g0[t] for _, _, t in modes], B)
   g_rows, _ = O.bucketize(ids, mode_l, nb_l, off_l)
   want = full.numpy()[g_rows].reshape(F, B, D).transpose(1, 0, 2).reshape(B, F * D)
-  assert np.array_equal(out.detach().numpy()[:, :F * D], want), 'sharded forward differs'
+  assert np.array_equal(out.numpy()[:, :F * D], want), 'sharded forward differs'
   gout = rng.normal(0, 0.1, (B, out.shape[1])).astype(np.float32)
   out.grad = torch.from_numpy(gout)
-  sa.backward_update(K.make_opt(_lib.OPT_ADAGRAD, 0.05))
+  sl.backward_update(outs, K.make_opt(_lib.OPT_ADAGRAD, 0.05))
   all_rows, all_g = [None] * world, [None] * world
   dist.all_gather_object(all_rows, g_rows)
   dist.all_gather_object(all_g, gout[:, :F * D].reshape(B, F, D).transpose(1, 0, 2).reshape(F * B, D))
@@ -104,19 +83,18 @@ def _worker(rank, port, ret, world):
                   grad_scale=1.0 / world)
   touched = 0
   for name, v in tables:
-    off, local, _ = sa.arena.tables[name]
-    g0 = 0 if name == 't0' else 101
-    want_shard = t[g0:g0 + v][rank::world]
-    got = sa.arena.weight[off:off + want_shard.shape[0]].numpy()
+    off = arena.tables[name][0]
+    want_shard = t[g0[name]:g0[name] + v][rank::world]
+    got = arena.weight[off:off + want_shard.shape[0]].numpy()
     np.testing.assert_allclose(got, want_shard, rtol=0, atol=1e-6)
-    touched += int((got != full.numpy()[g0:g0 + v][rank::world]).any())
+    touched += int((got != full.numpy()[g0[name]:g0[name] + v][rank::world]).any())
   ret[rank] = touched
   dist.destroy_process_group()
 
 
 @pytest.mark.timeout(600)
 @pytest.mark.parametrize('world', [2, 8])
-def test_row_sharded_arena_host_logic_gloo(world):
+def test_row_sharded_lookup_matches_unsharded_oracle_gloo(world):
   mgr = mp.Manager()
   ret = mgr.dict()
   mp.spawn(_worker, args=(_free_port(), ret, world), nprocs=world, join=True)
