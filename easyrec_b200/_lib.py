@@ -74,6 +74,8 @@ SIGNATURES = {
                                  c_vp]),
     'er_bucketize': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i32,
                              c_vp, c_vp, c_vp]),
+    'er_bucketize_weighted': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i32,
+                                      c_vp, c_vp, c_vp]),
     'er_dropout': (c_i32, [c_vp, c_i64, ctypes.c_float, ctypes.c_uint64, c_vp, c_vp, c_vp]),
     'er_gemm_small_workspace_bytes': (c_sz, [c_i64, c_i64, c_i64]),
     'er_gemm_small': (c_i32, [c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_sz,

@@ -44,11 +44,12 @@ struct BucketRule {  // 32 bytes, staged in shared memory per CTA
   int32_t seg_begin;
   int32_t mode;
   int32_t shard_n;
-  int32_t pad;
+  int32_t combiner;  // er_combiner without the ER_COMBINER_UNIT_WEIGHTS flag
 };
 
 __global__ void __launch_bounds__(256)
-    bucketize_kernel(const int64_t* __restrict__ ids, const int32_t* __restrict__ seg_ids,
+    bucketize_kernel(const int64_t* __restrict__ ids, const float* __restrict__ weights,
+                     const int32_t* __restrict__ seg_ids,
                      const int32_t* __restrict__ row_ptr, int64_t n_seg, int64_t cap,
                      const er_slot_t* __restrict__ slots, int n_slots,
                      int64_t* __restrict__ rows, int32_t* __restrict__ owner) {
@@ -64,7 +65,7 @@ __global__ void __launch_bounds__(256)
     r.seg_begin = s.seg_begin;
     r.mode = s.bucket_mode;
     r.shard_n = s.shard_n;
-    r.pad = 0;
+    r.combiner = s.combiner & 0xf;
     tab[i] = r;
     if (s.n_seg != nseg0 || s.seg_begin != i * nseg0) ok = 0;
   }
@@ -116,6 +117,9 @@ __global__ void __launch_bounds__(256)
       drop = (v < 0);
       r = v;
     }
+    // _prune_invalid_weights (compat/embedding_ops.py): a mean / sqrtn lookup whose weight is not > 0 (NaN included)
+    // is dropped here, so that K2, K7, er_mark_rows and K8 all see it as a dropped lookup
+    if (weights && tab[f].combiner != ER_COMBINER_SUM && !(weights[l] > 0.f)) drop = true;
     int32_t own = 0;
     if (shard_n > 1) {
       own = (int32_t)(r % shard_n);
@@ -153,10 +157,10 @@ extern "C" int er_csr_from_lens(const int32_t* lens, int64_t n_seg, int32_t* row
   return ER_OK;
 }
 
-extern "C" int er_bucketize(const int64_t* ids, const int32_t* seg_ids, const int32_t* row_ptr,
-                            int64_t n_seg, int64_t n_lookups_cap, const er_slot_t* slots,
-                            int32_t n_slots, int64_t* rows, int32_t* owner,
-                            er_stream_t stream) {
+extern "C" int er_bucketize_weighted(const int64_t* ids, const float* weights, const int32_t* seg_ids,
+                                     const int32_t* row_ptr, int64_t n_seg, int64_t n_lookups_cap,
+                                     const er_slot_t* slots, int32_t n_slots, int64_t* rows,
+                                     int32_t* owner, er_stream_t stream) {
   using namespace er;
   ER_REQUIRE(ids && rows && slots, "ids, rows and slots must be non-null");
   ER_REQUIRE(n_slots > 0 && n_slots <= 1024, "n_slots must be in [1, 1024]");
@@ -164,8 +168,16 @@ extern "C" int er_bucketize(const int64_t* ids, const int32_t* seg_ids, const in
   if (n_lookups_cap == 0) return ER_OK;
   cudaStream_t st = as_stream(stream);
   bucketize_kernel<<<grid_for(n_lookups_cap, 256, 8), 256, (size_t)n_slots * sizeof(BucketRule), st>>>(
-      ids, seg_ids, row_ptr, n_seg, n_lookups_cap, slots, n_slots, rows, owner);
+      ids, weights, seg_ids, row_ptr, n_seg, n_lookups_cap, slots, n_slots, rows, owner);
   count_launches(1);
   ER_CUDA_LAUNCH_CHECK();
   return ER_OK;
+}
+
+extern "C" int er_bucketize(const int64_t* ids, const int32_t* seg_ids, const int32_t* row_ptr,
+                            int64_t n_seg, int64_t n_lookups_cap, const er_slot_t* slots,
+                            int32_t n_slots, int64_t* rows, int32_t* owner,
+                            er_stream_t stream) {
+  return er_bucketize_weighted(ids, nullptr, seg_ids, row_ptr, n_seg, n_lookups_cap, slots, n_slots,
+                               rows, owner, stream);
 }

@@ -70,18 +70,17 @@ __global__ void __launch_bounds__(256)
       const SlotLite sl = slot_lite(sv, slot_of(sv, (int32_t)s));
       const int comb = slot_comb(sl);
       float4 o = f4_zero();
-      float scale = 0.f;
+      float scale = comb == ER_COMBINER_SUM ? 1.f : 0.f;   // sum: 1 for every segment, as the CSR and scalar paths
       const bool keep = r[u] >= 0 && (comb == ER_COMBINER_SUM || w[u] > 0.f);
       if (keep) {
         o = weights ? f4_scale(v[u], w[u]) : v[u];
-        scale = 1.f;
         if (comb == ER_COMBINER_MEAN) {
           o = f4_div(o, w[u]);
           scale = __fdiv_rn(1.f, w[u]);
         } else if (comb == ER_COMBINER_SQRTN) {
-          const float d = sqrtf(__fmul_rn(w[u], w[u]));
-          o = f4_div(o, d);
-          scale = __fdiv_rn(1.f, d);
+          const float d = sqrtf(__fmul_rn(w[u], w[u]));   // 0 when w*w underflows: zeros, as the CSR path
+          o = d != 0.f ? f4_div(o, d) : f4_zero();
+          scale = d != 0.f ? __fdiv_rn(1.f, d) : 0.f;
         }
       }
       float* dst = bufs.p[sl.misc & 0xff] + (int64_t)((int32_t)s - sl.seg_begin) * sl.out_stride + sl.out_col;
@@ -253,8 +252,8 @@ extern "C" int er_embedding_fwd(const float* table, int64_t n_rows, int32_t dim,
   }
   cudaStream_t st = as_stream(stream);
   const bool vec_dim = (dim == 4 || dim == 8 || dim == 16 || dim == 32 || dim == 64 || dim == 128);
-  // the host plan guarantees out_stride % 4 == 0 and out_col % 4 == 0 for vector dims; the
-  // scalar path has no alignment requirement.
+  // the host plan guarantees out_stride % 4 == 0 and out_col % 4 == 0 for vector dims
+  // (K.make_slots refuses other plans); the scalar path has no alignment requirement.
   if (vec_dim && aligned) {
     switch (dim / 4) {
       case 1: launch_vec<1>(table, row_stride, rows, weights, row_ptr, n_seg, n_lookups_cap, slots, n_slots, bufs, seg_scale, st); break;

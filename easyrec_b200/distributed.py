@@ -48,7 +48,7 @@ class GlobalCall(object):
                          out_col=int(s['out_col']) + r * rows_of_buf * int(s['out_stride']),
                          shard_n=1))
     assert max(r['out_col'] for r in recs) < 2**31
-    self.slots_np = K.make_slots(recs)
+    self.slots_np = K.make_slots(recs, call.arena.dim)
     dev = call.arena.device
     self.slots_dev = K.slots_to_device(self.slots_np, dev)
     self.n_slots = len(recs)

@@ -148,7 +148,7 @@ class ArenaCall(object):
                        out_stride=stride, out_col=col, shard_n=arena.shard_n))
       seg += n_seg
     self.n_seg = seg
-    self.slots_np = K.make_slots(recs)
+    self.slots_np = K.make_slots(recs, dim)
     self.slots_dev = K.slots_to_device(self.slots_np, arena.device)
     self.n_slots = len(recs)
     self.single_valued = single_valued

@@ -120,7 +120,7 @@ class MergedCall(object):
       seg += c.n_seg
       lookups += c.max_lookups
     assert len(self.buf_of) <= _lib.MAX_BUFS, 'too many output matrices on one arena'
-    self.slots_np = K.make_slots(recs)
+    self.slots_np = K.make_slots(recs, arena.dim)
     self.slots_dev = K.slots_to_device(self.slots_np, arena.device)
     self.n_slots = len(recs)
     self.n_seg = seg
@@ -801,7 +801,7 @@ class InputLayer(object):
       return rows, weights, row_ptr, seg_ids, outs
     rows = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
     K.bucketize(ids_cap, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr,
-                rows=rows)
+                rows=rows, **K.k1_weight_args(ids_cap, weights))
     outs = E.fused_lookup(call, rows, weights=weights, row_ptr=row_ptr)
     return rows, weights, row_ptr, seg_ids, outs
 

@@ -49,8 +49,15 @@ def _buf_array(bufs):
   return arr
 
 
-def make_slots(records):
-  """records: list of dicts with er_slot_t field names -> numpy structured array."""
+VECTOR_DIMS = (4, 8, 16, 32, 64, 128)
+
+
+def make_slots(records, dim=None):
+  """records: list of dicts with er_slot_t field names -> numpy structured array.
+
+  dim: the arena's embedding dim.  At the vector dims K2 and K7 move rows with 16-byte accesses at
+  out_stride * s + out_col of the slot's output buffer, so every out_stride and out_col must then be a multiple of 4
+  (include/er_b200.h); the slot table lives in device memory, where the kernels cannot check it."""
   arr = np.zeros(len(records), dtype=SLOT_DTYPE)
   for i, r in enumerate(records):
     for k, v in r.items():
@@ -60,6 +67,11 @@ def make_slots(records):
   order = np.argsort(arr['seg_begin'], kind='stable')
   if not np.array_equal(order, np.arange(len(records))):
     raise _lib.ErError('slots must be ordered by seg_begin')
+  if dim in VECTOR_DIMS:
+    bad = np.nonzero((arr['out_stride'] % 4 != 0) | (arr['out_col'] % 4 != 0))[0]
+    if bad.size:
+      raise _lib.ErError('slot %d: out_stride %d / out_col %d must be multiples of 4 at dim %d' % (
+          bad[0], arr[bad[0]]['out_stride'], arr[bad[0]]['out_col'], dim))
   return arr
 
 
@@ -85,19 +97,35 @@ def csr_from_lens(lens, n_lookups_cap, want_seg_ids=True):
 
 
 def bucketize(ids, slots_dev, n_slots, n_seg, seg_ids=None, row_ptr=None, rows=None,
-              owner=None):
+              owner=None, weights=None):
+  """K1 (er_bucketize).  weights: the lookup weights the lookup will be pooled with (er_bucketize_weighted); mean /
+  sqrtn lookups whose weight is not > 0 come out as dropped rows (-1), as safe_embedding_lookup_sparse prunes them."""
   lib = _lib.load()
   _chk(ids, torch.int64, 'ids')
+  _chk(weights, torch.float32, 'weights')
   _chk(seg_ids, torch.int32, 'seg_ids')
   _chk(row_ptr, torch.int32, 'row_ptr')
   _chk(owner, torch.int32, 'owner')
   if rows is None:
     rows = torch.empty_like(ids)
   _chk(rows, torch.int64, 'rows')
+  if weights is None:
+    _lib.check(
+        lib.er_bucketize(_p(ids), _p(seg_ids), _p(row_ptr), n_seg, ids.numel(), _p(slots_dev),
+                         n_slots, _p(rows), _p(owner), _stream()), 'er_bucketize')
+    return rows
+  assert weights.numel() >= ids.numel()
   _lib.check(
-      lib.er_bucketize(_p(ids), _p(seg_ids), _p(row_ptr), n_seg, ids.numel(), _p(slots_dev),
-                       n_slots, _p(rows), _p(owner), _stream()), 'er_bucketize')
+      lib.er_bucketize_weighted(_p(ids), _p(weights), _p(seg_ids), _p(row_ptr), n_seg, ids.numel(),
+                                _p(slots_dev), n_slots, _p(rows), _p(owner), _stream()), 'er_bucketize_weighted')
   return rows
+
+
+def k1_weight_args(ids, weights):
+  """Keyword arguments of bucketize() that hand a weighted CSR call's lookup weights to K1, so that the lookups the
+  pooling prunes are dropped before K7, er_mark_rows and K8 see them.  Only device tensors take this path: the host
+  runs of the input layer (tests/host_doubles.py) stand in for K1 with a double whose bucketize takes no weights."""
+  return {'weights': weights} if weights is not None and ids.is_cuda else {}
 
 
 def dropout(x, rate, seed, counter, out=None):

@@ -106,8 +106,9 @@ class ShardedExchange(object):
     if self._pre is not None:
       torch.cuda.current_stream().wait_stream(self._pre)
 
-  def lookup(self, first, ids, seg_ids=None, row_ptr=None):
-    """K1 -> K8 -> all_to_all(ids) -> every member's K2 on the owner -> ONE all_to_all(rows)."""
+  def lookup(self, first, ids, seg_ids=None, row_ptr=None, weights=None):
+    """K1 -> K8 -> all_to_all(ids) -> every member's K2 on the owner -> ONE all_to_all(rows).  weights: the lookup
+    weights of a CSR call (K1 drops the mean / sqrtn lookups they prune, so K8 does not request those rows)."""
     N = self.world
     call = first.call
     if seg_ids is not None:
@@ -126,7 +127,7 @@ class ShardedExchange(object):
       self._have_next = False
     else:
       K.bucketize(ids, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr, rows=self.rows_local,
-                  owner=self.owner)
+                  owner=self.owner, **K.k1_weight_args(ids, weights))
       K.shard_group(self.rows_local, self.owner, N, self.cap, self.send_rows, self.pos, self.counts, self.group_ws)
       self.overflow += self.counts[N:]
       dist.all_to_all_single(self.recv_rows, self.send_rows)
@@ -216,12 +217,12 @@ class ShardedLookup(object):
       recs.append(dict(num_buckets=self.n_ex, row_offset=0, seg_begin=int(r['seg_begin']), n_seg=int(r['n_seg']),
                        bucket_mode=mode, combiner=int(r['combiner']), out_buf=int(r['out_buf']),
                        out_stride=int(r['out_stride']), out_col=int(r['out_col']), shard_n=1))
-    self.pool_slots_np = K.make_slots(recs)
+    self.pool_slots_np = K.make_slots(recs, D)
     self.pool_slots = K.slots_to_device(self.pool_slots_np, dev)
     own = [dict(num_buckets=a.n_rows, row_offset=0, seg_begin=0, n_seg=self.n_ex, bucket_mode=_lib.BUCKET_NONE,
                 combiner=_lib.COMBINER_SUM | _lib.COMBINER_UNIT_WEIGHTS, out_buf=0, out_stride=W, out_col=self.col,
                 shard_n=1)]
-    self.owner_slots = K.slots_to_device(K.make_slots(own), dev)
+    self.owner_slots = K.slots_to_device(K.make_slots(own, D), dev)
     self.owner_ws = K.bwd_workspace(self.n_ex, dev, D)
     self.pool_ws = K.bwd_workspace(self.L, dev, D)
     self.recv_view = ex.recv_emb[:, self.col:self.col + D]   # this arena's received rows: the pooling K2's "table"
@@ -235,7 +236,7 @@ class ShardedLookup(object):
     ex.build()
     assert (row_ptr is not None) == self.csr
     if ids is not None:
-      ex.lookup(self, ids, seg_ids=seg_ids, row_ptr=row_ptr)
+      ex.lookup(self, ids, seg_ids=seg_ids, row_ptr=row_ptr, weights=weights if self.csr else None)
     K.embedding_fwd(self.recv_view, call.arena.dim, ex.pos, self.pool_slots, call.n_slots, call.n_seg, outs, weights=weights,
                     row_ptr=row_ptr, seg_scale=call.seg_scale)
     self._weights = weights

@@ -153,13 +153,24 @@ int er_csr_from_lens(const int32_t* lens, int64_t n_seg, int32_t* row_ptr,
 /* ---- K1: raw ids -> arena rows ---------------------------------------
  * rows[l] = slot.row_offset + bucket(ids[l]) per the slot's er_bucket_mode,
  * or -1 when the lookup is dropped.  With shard_n > 1 the result is the
- * owner-local row and owner[l] (may be NULL) receives id mod shard_n.
+ * owner-local row and owner[l] (may be NULL) receives id mod shard_n
+ * (-1 for a dropped lookup).
  * seg_ids == NULL means lookup l belongs to segment l (single-valued slots);
  * row_ptr == NULL means exactly n_lookups_cap lookups, else row_ptr[n_seg]. */
 int er_bucketize(const int64_t* ids, const int32_t* seg_ids,
                  const int32_t* row_ptr, int64_t n_seg, int64_t n_lookups_cap,
                  const er_slot_t* slots, int32_t n_slots, int64_t* rows,
                  int32_t* owner, er_stream_t stream);
+/* er_bucketize given the lookup weights that K2 and K7 will be given (NULL:
+ * the same as er_bucketize).  A lookup of a mean / sqrtn slot whose weight is
+ * not > 0 (NaN included) is dropped here (safe_embedding_lookup_sparse's
+ * _prune_invalid_weights, compat/embedding_ops.py), so that K2, K7,
+ * er_mark_rows and K8 agree that its row is not looked up; sum slots keep
+ * every weight.  Weighted calls with mean / sqrtn slots must use this form. */
+int er_bucketize_weighted(const int64_t* ids, const float* weights, const int32_t* seg_ids,
+                          const int32_t* row_ptr, int64_t n_seg, int64_t n_lookups_cap,
+                          const er_slot_t* slots, int32_t n_slots, int64_t* rows,
+                          int32_t* owner, er_stream_t stream);
 
 /* ---- K8: index bucketing of the row-sharded lookup --------------------
  * Replaces the Unique + dynamic_partition + host-read split sizes of
@@ -189,8 +200,19 @@ uint64_t er_fingerprint64_host(const char* s, size_t len);
  *   out_bufs[slot.out_buf][(s-slot.seg_begin)*out_stride + out_col + 0..dim)
  * i.e. the per-group concat of feature_column.input_layer
  * (compat/feature_column/feature_column.py:384-414) is fused into the store.
+ * Inside a segment the terms w_l * row are added in lookup order, with
+ * separate multiply and add (no FMA contraction).
  * seg_scale (n_seg floats, may be NULL when every slot is sum) receives the
- * mean/sqrtn denominators' reciprocal for the backward pass.
+ * mean/sqrtn denominators' reciprocal for the backward pass: 1/sum w for mean,
+ * 1/sqrt(sum w^2) for sqrtn, 0 for an empty (or wholly pruned) mean / sqrtn
+ * segment, and exactly 1 for every segment of a sum slot, empty ones included.
+ * Lookups past min(n_lookups_cap, row_ptr[n_seg]) are not read.
+ * At dim 4, 8, 16, 32, 64 and 128 (when table, row_stride and every out_bufs
+ * base are 16-byte aligned) rows are moved with 16-byte accesses at
+ * out_bufs[out_buf] + s*out_stride + out_col, and er_embedding_bwd reads
+ * grad_bufs the same way: every slot's out_stride and out_col must then be
+ * multiples of 4.  The slot table is device memory, so the kernels cannot
+ * check this; the host-side plan builders refuse plans that break it.
  * out_bufs is a HOST array of n_bufs (<= ER_MAX_BUFS) device pointers. */
 int er_embedding_fwd(const float* table, int64_t n_rows, int32_t dim,
                      int32_t row_stride, const int64_t* rows,
@@ -213,7 +235,10 @@ int er_embedding_fwd(const float* table, int64_t n_rows, int32_t dim,
  * bucket that a whole CTA sorts.  When uniq_rows is given and dim is 1 or a
  * vector width up to 32, shorter runs are also summed by a fixed tree (a
  * warp's shuffle scan).  Slots of mode ER_BUCKET_ONE_ROW take a weighted
- * column sum instead.  state0/state1: adagrad accumulator | adam m, v (same
+ * column sum instead.  Every lookup with rows[l] >= 0 counts as touching its
+ * row (even with a zero coefficient), so rows must already carry -1 for the
+ * lookups safe_embedding_lookup_sparse prunes: er_bucketize_weighted given
+ * the same weights does that.  state0/state1: adagrad accumulator | adam m, v (same
  * layout and stride as table; unused ones NULL).
  * When uniq_rows/uniq_grads are non-NULL the deduplicated gradient is ALSO
  * written there (compact, sorted by row; *n_uniq receives the count); pass

@@ -56,6 +56,25 @@ def test_gemm_refuses_pitch_shorter_than_row_without_gpu():
     assert st == _lib.ER_ERR_INVALID_ARG and b'pitch smaller than row' in lib.er_last_error()
 
 
+def test_make_slots_refuses_misaligned_vector_plans():
+  """At the vector dims K2 and K7 access out_bufs[out_buf] + s*out_stride + out_col 16 bytes at a time, so the plan
+  builder refuses an out_stride or out_col that is not a multiple of 4 there; scalar dims take any plan."""
+  from easyrec_b200 import kernels as K
+
+  def rec(stride, col):
+    return [dict(num_buckets=10, row_offset=0, seg_begin=0, n_seg=4, bucket_mode=_lib.BUCKET_NONE, out_buf=0,
+                 out_stride=stride, out_col=col)]
+
+  for dim in K.VECTOR_DIMS:
+    K.make_slots(rec(4 * dim, dim), dim)
+    for stride, col in ((4 * dim + 2, 0), (4 * dim, 2), (4 * dim + 1, 3)):
+      with pytest.raises(_lib.ErError, match='multiples of 4'):
+        K.make_slots(rec(stride, col), dim)
+  for dim in (1, 3, 6, 12):
+    K.make_slots(rec(4 * dim + 1, 3), dim)
+  K.make_slots(rec(18, 2))   # no dim: not checked
+
+
 def test_product_never_imports_oracle():
   pkg = os.path.join(ROOT, 'easyrec_b200')
   for dp, _, files in os.walk(pkg):
