@@ -158,6 +158,9 @@ SIGNATURES = {
     'er_din_concat_bwd': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp]),
     'er_din_pool_fwd': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp]),
     'er_din_pool_bwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp]),
+    'er_din_sigmoid_pool_fwd': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_f32, c_vp, c_vp, c_vp]),
+    'er_din_sigmoid_pool_bwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_f32, c_vp, c_vp, c_i32,
+                                        c_vp]),
     'er_cross_fwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp]),
     'er_cross_workspace_bytes': (c_sz, [c_i64, c_i32]),
     'er_cross_bwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32,

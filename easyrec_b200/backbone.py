@@ -309,6 +309,83 @@ def regularised_groups(backbone_config):
   return sorted(out)
 
 
+def seq_output_groups(backbone_config):
+  """feature groups read by `input_layer { output_seq_and_normal_feature: true }` blocks
+  (layers/common_layers.py:104-131).  The (seq, seq_len, target) triple of such a block feeds keras `DIN` blocks
+  only; a group read this way is read no other way, since its sequence features are looked up un-pooled."""
+  blocks = list(backbone_config.blocks) + [b for p in backbone_config.packages for b in p.blocks]
+  seq_blocks, groups, other = set(), set(), set()
+  for b in blocks:
+    reads = [inp.feature_group_name for inp in b.inputs if inp.WhichOneof('name') == 'feature_group_name']
+    if b.WhichOneof('layer') == 'input_layer' and b.input_layer.output_seq_and_normal_feature:
+      if not b.input_layer.concat_seq_feature:
+        raise NotImplementedError('input_layer block %s: concat_seq_feature: false (DIN takes the concatenated '
+                                  'sequence)' % b.name)
+      seq_blocks.add(b.name)
+      groups.update(reads)
+    else:
+      other.update(reads)
+  both = groups & other
+  if both:
+    raise NotImplementedError('feature group(s) %s read by output_seq_and_normal_feature and by another block'
+                              % sorted(both))
+  for b in blocks:
+    if not any(inp.WhichOneof('name') == 'block_name' and inp.block_name in seq_blocks for inp in b.inputs):
+      continue
+    cls = b.keras_layer.class_name if b.WhichOneof('layer') == 'keras_layer' else b.WhichOneof('layer')
+    if cls != 'DIN':
+      raise NotImplementedError('backbone block %s (%s) reads the sequence output of output_seq_and_normal_feature: '
+                                'only DIN blocks are built over it' % (b.name, cls))
+  return groups
+
+
+class DIN(nn.Module):
+  """keras DIN block (layers/keras/din.py:16-67) over the (seq, seq_len, target) triple of an
+  output_seq_and_normal_feature input layer: [q, k, q-k, q*k] over the T steps -> attention MLP (use_final_bn off,
+  final bias on, linear final activation forced; BN / dice statistics over all B*T rows) -> scores masked beyond the
+  length -> softmax, or sigmoid(s / sqrt(seq width)) -> weighted sum of the keys [-> | target].  A target narrower
+  than the history is zero-padded to its width; the pooled vector then keeps the target's width."""
+
+  def __init__(self, seq_width, query_width, conf, generator=None):
+    super().__init__()
+    if query_width is None:
+      raise ValueError('[DIN] target feature is empty (the sequence group has no plain features)')
+    if query_width > seq_width:
+      raise ValueError('DIN: the embedding size of target item (%d) is larger than the one of sequence (%d)'
+                       % (query_width, seq_width))
+    if conf.attention_normalizer not in ('softmax', 'sigmoid'):
+      raise ValueError('unsupported attention normalizer: ' + conf.attention_normalizer)
+    mlp_conf = type(conf.attention_dnn)()
+    mlp_conf.CopyFrom(conf.attention_dnn)
+    mlp_conf.use_final_bn = False
+    mlp_conf.use_final_bias = True
+    mlp_conf.final_activation = 'linear'
+    self.mlp = MLP(4 * seq_width, mlp_conf, generator)
+    if self.mlp.out_dim != 1:
+      raise NotImplementedError('DIN attention_dnn must end in one unit (has %d)' % self.mlp.out_dim)
+    self.sigmoid = conf.attention_normalizer == 'sigmoid'
+    self.need_target = bool(conf.need_target_feature)
+    self.seq_width, self.query_width = seq_width, query_width
+    self.out_dim = query_width + (seq_width if self.need_target else 0)
+
+  def forward(self, inputs):
+    keys, lens, query = inputs
+    B, T, D = keys.shape
+    if self.query_width < D:
+      query = torch.nn.functional.pad(query, (0, D - self.query_width))
+    query, keys = query.contiguous(), keys.contiguous()
+
+    def mlp(din_in):
+      return self.mlp(din_in.reshape(B * T, 4 * D))
+    if self.sigmoid:
+      att = I.din_sigmoid_attention(query, keys, lens, mlp, 1.0 / math.sqrt(D))
+    else:
+      att = I.din_attention(query, keys, lens, mlp)
+    if self.query_width < D:
+      att = att[:, :self.query_width]   # = the pool over keys[:, :, :query_width]: columns are summed independently
+    return torch.cat([att, query], dim=1) if self.need_target else att
+
+
 class Backbone(nn.Module):
   """Backbone.__call__ + Package.call (backbone.py:215-348,482-510).  Layers are instantiated by a shape-only
   dry run on `meta` tensors, so construction needs no GPU and the optimizer sees every parameter."""
@@ -390,6 +467,11 @@ class Backbone(nn.Module):
           params = {k: (v.bool_value if v.HasField('bool_value') else v.number_value)
                     for k, v in conf.st_params.fields.items()}
         self.mods[name] = DotInteraction(params)
+      elif cls == 'DIN':
+        if not (isinstance(x, (list, tuple)) and len(x) == 3 and x[0].dim() == 3):
+          raise NotImplementedError('DIN block %s takes the (seq, seq_len, target) output of an input_layer block with '
+                                    'output_seq_and_normal_feature' % name)
+        self.mods[name] = DIN(x[0].shape[-1], None if x[2] is None else x[2].shape[-1], conf.din, self._gen)
       else:
         raise NotImplementedError('backbone keras_layer %s' % cls)
     mod = self.mods[name]
@@ -410,6 +492,8 @@ class Backbone(nn.Module):
       if isinstance(mod, DotInteraction):
         n = len(x) if isinstance(x, (list, tuple)) else first.shape[1]
         return torch.empty((first.shape[0], mod.out_dim(n)), device='meta')
+      if isinstance(mod, DIN):
+        return torch.empty((first.shape[0], mod.out_dim), device='meta')
     return mod(x)
 
   def _layer(self, name, conf, x, build):
@@ -466,15 +550,29 @@ class Backbone(nn.Module):
         return torch.empty(batch_size, width, device='meta')
       return list(group_tensors[name][1]) if as_list else group_tensors[name][0]
 
+    def seq_group(name):
+      # EnhancedInputLayer with output_seq_and_normal_feature (layers/common_layers.py:104-131): (seq [B, T, sum D],
+      # lengths of the first sequence feature, plain features concatenated or None)
+      if build:
+        sl = il.seq_group_layout[name]
+        tw = sum(e[2] for e in il.group_layout[name])
+        return (torch.empty(batch_size, sl['T'], sum(e[1] for e in sl['seq']), device='meta'),
+                torch.empty(batch_size, dtype=torch.int32, device='meta'),
+                torch.empty(batch_size, tw, device='meta') if il.group_layout[name] else None)
+      return group_tensors[name][:3]
+
     outputs = {}
     for block in self.blocks:
       which = block.WhichOneof('layer')
       # EnhancedInputLayer.call (layers/common_layers.py:142-190): the group as one matrix, as its feature list,
       # as a [B, F, D] stack, or as the (matrix, list) pair that later blocks pick apart with input_slice
       ilc = block.input_layer if which == 'input_layer' else None
-      mode = 'list' if ilc and ilc.only_output_feature_list else '3d' if ilc and ilc.only_output_3d_tensor else \
+      mode = 'seq' if ilc and ilc.output_seq_and_normal_feature else \
+          'list' if ilc and ilc.only_output_feature_list else '3d' if ilc and ilc.only_output_3d_tensor else \
           'both' if ilc and ilc.output_2d_tensor_and_feature_list else '2d'
-      if mode == '2d':
+      if mode == 'seq':
+        getter = seq_group
+      elif mode == '2d':
         getter = groups
       elif mode == 'list':
         getter = lambda n: groups(n, True)  # noqa: E731
@@ -491,7 +589,8 @@ class Backbone(nn.Module):
         continue
       x = self._block_input(block, outputs, getter)
       if which == 'input_layer':
-        if any(0.0 < r < 1.0 for r in (ilc.dropout_rate, ilc.feature_dropout_rate)) or ilc.do_batch_norm or ilc.do_layer_norm:
+        # (the sequence output returns before dropout / normalisation are applied, common_layers.py:103-105)
+        if mode != 'seq' and any(0.0 < r < 1.0 for r in (ilc.dropout_rate, ilc.feature_dropout_rate)) or ilc.do_batch_norm or ilc.do_layer_norm:
           raise NotImplementedError('input_layer block %s: dropout / feature dropout / normalisation' % block.name)
         out = x
       elif which in ('keras_layer', 'lambda', 'recurrent', 'repeat'):

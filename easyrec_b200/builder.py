@@ -309,6 +309,8 @@ def build_model(pipeline_config, batch_size, device, generator=None, cpu_generat
   opt = optimizer_settings(pipeline_config)
   cls = model_pkg.get_model_class(mc.model_class)
   wide_dim = cls.wide_output_dim(mc)
+  from easyrec_b200 import backbone
+  seq_groups = backbone.seq_output_groups(mc.backbone) if mc.HasField('backbone') else set()
   if generator is None and not str(device).startswith('cuda'):
     generator = cpu_generator   # tables initialised from the caller's seed on a host build too
   il = IL.InputLayer(specs, groups, batch_size, device, wide_output_dim=wide_dim,
@@ -323,7 +325,8 @@ def build_model(pipeline_config, batch_size, device, generator=None, cpu_generat
                      seq_combiners={(fc.feature_name if fc.HasField('feature_name') else fc.input_names[0]):
                                     fc.sequence_combiner.WhichOneof('combiner')
                                     for fc in config_util.get_feature_configs(pipeline_config)
-                                    if fc.HasField('sequence_combiner')})
+                                    if fc.HasField('sequence_combiner')},
+                     seq_output_groups=seq_groups)
   il.pad_tags = pad_tags   # tag features of a backbone `embedding_layer` block: the readers pad them with the bucket of ''
   # RawFeature.normalizer_fn: applied to the min-max normalised value on the device (input/input.py:642-646); the
   # readers apply the same function on the host to raw features they bucketize themselves (readers.bucketize_raw)

@@ -130,6 +130,57 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// attention_normalizer 'sigmoid' of the keras DIN block (layers/keras/din.py:57-60):
+// p[b,t] = t < len ? sigmoid(scale * s[b,t]) : 0 (the masked score -2^32+1 gives exactly 0 in fp32 there),
+// out[b,:] = sum_t p[b,t] * keys[b,t,:] in ascending t.  One warp per sample.
+__global__ void __launch_bounds__(256)
+    din_sigmoid_pool_fwd_kernel(const float* __restrict__ scores, const float* __restrict__ keys,
+                                const int32_t* __restrict__ lens, int64_t batch, int seq_len, int dim,
+                                float scale, float* __restrict__ probs, float* __restrict__ out) {
+  er_pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= batch) return;
+  const int len = lens ? lens[b] : seq_len;
+  for (int t = lane; t < seq_len; t += 32)
+    probs[b * seq_len + t] = t < len ? 1.0f / (1.0f + expf(-scale * scores[b * seq_len + t])) : 0.f;
+  __syncwarp();
+  for (int d = lane; d < dim; d += 32) {
+    float acc = 0.f;
+    for (int t = 0; t < seq_len; ++t) acc += probs[b * seq_len + t] * keys[(b * seq_len + t) * dim + d];
+    out[b * dim + d] = acc;
+  }
+}
+
+// g_score[t] = t < len ? scale * p (1 - p) * (gout . keys[t]) : 0 ; g_keys[t,:] (+)= p[t] * gout
+__global__ void __launch_bounds__(256)
+    din_sigmoid_pool_bwd_kernel(const float* __restrict__ probs, const float* __restrict__ keys,
+                                const float* __restrict__ gout, const int32_t* __restrict__ lens, int64_t batch,
+                                int seq_len, int dim, float scale, float* __restrict__ g_scores,
+                                float* __restrict__ g_keys, int accumulate_gkeys) {
+  er_pdl_wait();
+  const int lane = threadIdx.x & 31;
+  const int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= batch) return;
+  const int len = lens ? lens[b] : seq_len;
+  for (int t = 0; t < seq_len; ++t) {
+    const float p = probs[b * seq_len + t];
+    float dp = 0.f;
+    for (int d = lane; d < dim; d += 32) {
+      const int64_t i = (b * seq_len + t) * dim + d;
+      const float g = gout[b * dim + d];
+      dp += g * keys[i];
+      const float v = p * g;
+      if (accumulate_gkeys)
+        g_keys[i] += v;
+      else
+        g_keys[i] = v;
+    }
+    dp = warp_sum(dp);
+    if (lane == 0) g_scores[b * seq_len + t] = t < len ? scale * p * (1.0f - p) * dp : 0.f;
+  }
+}
+
 // ---- DCN v1 cross layer ------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
     cross_fwd_kernel(const float* __restrict__ x0, const float* __restrict__ xl, const float* __restrict__ w,
@@ -400,6 +451,31 @@ extern "C" int er_din_pool_bwd(const float* probs, const float* keys, const floa
   ER_REQUIRE(batch > 0 && seq_len > 0 && dim > 0, "bad shape");
   din_pool_bwd_kernel<<<warps_grid(batch), 256, 0, as_stream(stream)>>>(
       probs, keys, gout, lens, batch, seq_len, dim, g_scores, g_keys, accumulate_gkeys);
+  count_launches(1);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_din_sigmoid_pool_fwd(const float* scores, const float* keys, const int32_t* lens,
+                                       int64_t batch, int32_t seq_len, int32_t dim, float scale, float* probs,
+                                       float* out, er_stream_t stream) {
+  ER_REQUIRE(scores && keys && probs && out, "null argument");
+  ER_REQUIRE(batch > 0 && seq_len > 0 && dim > 0, "bad shape");
+  launch_pdl(din_sigmoid_pool_fwd_kernel, dim3(warps_grid(batch)), dim3(256), 0, as_stream(stream), scores, keys,
+             lens, batch, seq_len, dim, scale, probs, out);
+  count_launches(1);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_din_sigmoid_pool_bwd(const float* probs, const float* keys, const float* gout,
+                                       const int32_t* lens, int64_t batch, int32_t seq_len, int32_t dim,
+                                       float scale, float* g_scores, float* g_keys, int32_t accumulate_gkeys,
+                                       er_stream_t stream) {
+  ER_REQUIRE(probs && keys && gout && g_scores && g_keys, "null argument");
+  ER_REQUIRE(batch > 0 && seq_len > 0 && dim > 0, "bad shape");
+  launch_pdl(din_sigmoid_pool_bwd_kernel, dim3(warps_grid(batch)), dim3(256), 0, as_stream(stream), probs, keys,
+             gout, lens, batch, seq_len, dim, scale, g_scores, g_keys, (int)accumulate_gkeys);
   count_launches(1);
   ER_CUDA_LAUNCH_CHECK();
   return ER_OK;

@@ -156,8 +156,11 @@ class InputLayer(object):
   def __init__(self, features, groups, batch_size, device, wide_output_dim=1,
                embedding_optimizer=_lib.OPT_ADAGRAD, shard_n=1, shard_rank=0, generator=None,
                adagrad_init=0.1, seq_att_groups=None, max_tag_lookups=None, uniform_tables=None,
-               dense_generator=None, multi_valued_seq=(), seq_combiners=None):
+               dense_generator=None, multi_valued_seq=(), seq_combiners=None, seq_output_groups=()):
     self.features = collections.OrderedDict((f.name, f) for f in features)
+    # groups read only by backbone `input_layer { output_seq_and_normal_feature: true }` blocks
+    # (layers/common_layers.py:104-131): their SequenceFeatures come out un-pooled as one [B, T, sum D] tensor
+    self.seq_output_groups = set(seq_output_groups)
     # SequenceFeatures with seq_multi_sep: every step holds a LIST of values, pooled per step by the feature's
     # combiner (input/input.py:686-700 builds the 3-D SparseTensor; pinned by test/embed_test.py:88-151) - a CSR slot
     # with one segment per (sample, step) instead of one id per step
@@ -184,6 +187,7 @@ class InputLayer(object):
     self.subcalls = collections.OrderedDict()        # dim -> OrderedDict(key -> _SubCall)
     self.group_layout = {}    # group -> list of (feature, kind, width, dim, out_key, col)
     self.seq_layout = {}      # seq group -> dict(key=[(feature, dim, out_key, col)], hist=[...], T=..)
+    self.seq_group_layout = {}   # output_seq_and_normal_feature group -> dict(seq=[(feature, dim, out_key, col)], T=..)
 
     def add_slot(dim, out_key, fname, table, kind, wide=False, pooled_seq=False):
       f = self.features[fname]
@@ -221,11 +225,34 @@ class InputLayer(object):
       layout = []
       seqc = []
       wide = bool(g.get('wide'))
+      if gname in self.seq_output_groups:
+        if wide:
+          raise NotImplementedError('feature group %s: wide_deep WIDE read by output_seq_and_normal_feature' % gname)
+        if g.get('seq'):
+          raise NotImplementedError('feature group %s: sequence_features in a group read by '
+                                    'output_seq_and_normal_feature' % gname)
+        self.seq_group_layout[gname] = dict(seq=[], T=None)
       for fname in g['features']:
         f = self.features[fname]
         dim = wide_output_dim if wide else f.embedding_dim
         if f.kind == 'raw' and dim == 0:
           layout.append((fname, 'dense', f.raw_input_dim, None, None, None))
+          continue
+        if f.kind == 'seq' and gname in self.seq_output_groups:
+          # InputLayer.get_sequence_feature (layers/input_layer.py:154-192): the un-pooled [B, T, D] lookup, in the
+          # table of the column itself (variable_scope('input_layer/' + column name): no group scope, so a feature
+          # listed in another group too reads the same table).  T is max_seq_len, fixed so the step can be captured.
+          sl = self.seq_group_layout[gname]
+          if fname in self.multi_valued_seq:
+            raise NotImplementedError('SequenceFeature %s: seq_multi_sep (multi-valued steps) in group %s read by '
+                                      'output_seq_and_normal_feature' % (fname, gname))
+          if sl['T'] not in (None, f.seq_len):
+            raise NotImplementedError('feature group %s: SequenceFeatures of different max_seq_len (%d, %d) read by '
+                                      'output_seq_and_normal_feature' % (gname, sl['T'], f.seq_len))
+          sl['T'] = f.seq_len
+          # all sequence features of one width write one [B*T, sum D] matrix: the concat costs nothing
+          add_slot(dim, gname + '#seq', fname, f.embedding_name or fname + '_embedding', 'seq')
+          sl['seq'].append([fname, dim, gname + '#seq', None])
           continue
         if f.kind == 'seq':
           if self.seq_combiners.get(fname) != 'attention' or wide or fname in self.multi_valued_seq:
@@ -252,6 +279,8 @@ class InputLayer(object):
         layout.append([fname, 'emb', dim, dim, out_key, None])
       self.seqc_order[gname] = [e[0] for e in seqc]
       self.group_layout[gname] = layout + sorted(seqc, key=lambda e: e[0])
+      if gname in self.seq_group_layout and not self.seq_group_layout[gname]['seq']:
+        raise ValueError('[input_%s] sequence feature is empty (output_seq_and_normal_feature)' % gname)
     for sname, maps in self.seq_att_groups.items():
       lay = dict(key=[], hist=[], T=None)
       for keys, hists in maps:
@@ -361,9 +390,9 @@ class InputLayer(object):
             for e in lay:
               if e[1] in ('emb', 'seqc') and e[0] == fname and e[4] == out_key and e[5] is None:
                 e[5] = col
-          for lay in self.seq_layout.values():
-            for part in ('key', 'hist'):
-              for e in lay[part]:
+          for lay in list(self.seq_layout.values()) + list(self.seq_group_layout.values()):
+            for part in ('key', 'hist', 'seq'):
+              for e in lay.get(part, ()):
                 if e[0] == fname and e[2] == out_key and e[3] is None:
                   e[3] = col
         for j, k in enumerate(keys):
@@ -825,6 +854,9 @@ class InputLayer(object):
       self._last_features = features
     if group_name in self.seq_layout:
       return self.seq_outputs[group_name]
+    if group_name in self.seq_group_layout:
+      raise NotImplementedError('feature group %s is read by output_seq_and_normal_feature blocks: lookup() returns its '
+                                '(seq, seq_len, target, plain features)' % group_name)
     concat, per_feature = self._last_groups[group_name]
     if not is_combine:
       return [], concat, per_feature
@@ -929,7 +961,9 @@ class InputLayer(object):
           v = mat[:, col:col + width]
         per_feature.append(v)
         kinds.append(kind)
-      if len(mats) == 1 and all(k == 'emb' for k in kinds):
+      if not layout:   # (only sequence features, read by output_seq_and_normal_feature)
+        concat = None
+      elif len(mats) == 1 and all(k == 'emb' for k in kinds):
         (dim, out_key), mat = next(iter(mats.items()))
         width = sum(e[2] for e in layout)
         concat = mat if mat.shape[1] == width else mat[:, :width]
@@ -944,5 +978,28 @@ class InputLayer(object):
         # the per-feature list keeps the sequence-combiner features in config order (the concat has them by name)
         by_name = {e[0]: v for e, v in zip(layout, per_feature) if e[1] == 'seqc'}
         per_feature = [v for e, v in zip(layout, per_feature) if e[1] != 'seqc'] + [by_name[n] for n in order]
+      if gname in self.seq_group_layout:
+        seq, seq_len = self._seq_group_tensors(gname, features, outs_by_key)
+        # the embedding regulariser covers the un-pooled sequence embeddings and the plain embedding columns
+        # (input_layer.py:117-151, 176-191)
+        seq._er_reg = [seq] + [v for v, k in zip(per_feature, kinds) if k == 'emb']
+        out[gname] = (seq, seq_len, concat, per_feature)
+        continue
       out[gname] = (concat, per_feature)
     return out
+
+  def _seq_group_tensors(self, gname, features, outs_by_key):
+    """EnhancedInputLayer.build (layers/common_layers.py:114-127) with concat_seq_feature: the group's sequence
+    features side by side on the last axis, [B, T, sum D], and the lengths of the FIRST of them."""
+    lay = self.seq_group_layout[gname]
+    B, T = self.batch_size, lay['T']
+    parts = []   # [matrix, first column, width]: neighbouring columns of one matrix are one view
+    for _, d, ok, c in lay['seq']:
+      mat = outs_by_key[(d, ok)]
+      if parts and parts[-1][0] is mat and parts[-1][1] + parts[-1][2] == c:
+        parts[-1][2] += d
+      else:
+        parts.append([mat, c, d])
+    views = [m[:, c:c + w].reshape(B, T, w) for m, c, w in parts]
+    seq = views[0] if len(views) == 1 else torch.cat(views, dim=-1)
+    return seq, features['seq_fea'][lay['seq'][0][0]][1]

@@ -131,6 +131,45 @@ def din_attention(query, keys, lens, attention_mlp):
   return _DinPool.apply(scores, keys, lens)
 
 
+class _DinSigmoidPool(torch.autograd.Function):
+  """p = sigmoid(scale * scores) on the first lens[b] steps, 0 beyond; weighted sum of the keys."""
+
+  @staticmethod
+  def forward(ctx, scores, keys, lens, scale):
+    scores, keys = _f32(scores), _f32(keys)
+    B, T, D = keys.shape
+    probs = torch.empty(B, T, dtype=torch.float32, device=keys.device)
+    out = torch.empty(B, D, dtype=torch.float32, device=keys.device)
+    _lib.check(_lib.load().er_din_sigmoid_pool_fwd(_p(scores), _p(keys), _p(lens), B, T, D, scale, _p(probs), _p(out),
+                                                   _stream()), 'er_din_sigmoid_pool_fwd')
+    ctx.save_for_backward(probs, keys, lens)
+    ctx.scale = scale
+    return out
+
+  @staticmethod
+  def backward(ctx, gout):
+    probs, keys, lens = ctx.saved_tensors
+    B, T, D = keys.shape
+    gs = torch.empty_like(probs)
+    gk = torch.empty_like(keys)
+    _lib.check(_lib.load().er_din_sigmoid_pool_bwd(_p(probs), _p(keys), _p(_f32(gout)), _p(lens), B, T, D, ctx.scale,
+                                                   _p(gs), _p(gk), 0, _stream()), 'er_din_sigmoid_pool_bwd')
+    return gs, gk, None, None
+
+
+def din_sigmoid_pool(scores, keys, lens, scale):
+  """sigmoid(scale * scores [B,T]) on the first lens[b] steps (0 beyond), weighted sum of keys [B,T,D] -> [B,D]: the
+  'sigmoid' attention_normalizer of the keras DIN block (layers/keras/din.py:57-60, scale = 1/sqrt(D))."""
+  return _DinSigmoidPool.apply(scores, keys, lens, float(scale))
+
+
+def din_sigmoid_attention(query, keys, lens, attention_mlp, scale):
+  """din_attention with the sigmoid normaliser: [q, k, q-k, q*k] -> attention_mlp -> din_sigmoid_pool."""
+  din_in = _DinConcat.apply(query, keys)
+  scores = attention_mlp(din_in).reshape(keys.shape[0], keys.shape[1])
+  return din_sigmoid_pool(scores, keys, lens, scale)
+
+
 class _Cross(torch.autograd.Function):
   """x_{l+1} = x0 * (x_l . w) + b + x_l."""
 

@@ -133,6 +133,32 @@ def c3_config_text(batch_size=4096, item_vocab=1_000_000, seq_len=50, optimizer=
   return text.encode()
 
 
+def c3_backbone_config_text(batch_size=4096, item_vocab=1_000_000, seq_len=50, optimizer='adagrad_optimizer', lr=0.01,
+                            normalizer='softmax'):
+  """C3's features (and c3_batch's batches) as the backbone DIN of samples/model_config/din_backbone_on_taobao.config:
+  user / item MLP blocks, an output_seq_and_normal_feature input layer over [item_id, cate_id | hist_items, hist_cates]
+  feeding a keras DIN block (attention MLP [128, 64, 32, 1] with dice, `normalizer`), top MLP [256, 128, 64].  The
+  target columns read the item group's tables; the histories have tables of their own."""
+  head = c3_config_text(batch_size, item_vocab, seq_len, optimizer, lr).split(b'model_config {')[0].decode()
+  mlp = 'keras_layer { class_name: "MLP" mlp { hidden_units: [128, 64] } }'
+  return (head + '\n'.join([
+      'model_config { model_class: "RankModel"',
+      '  feature_groups { group_name: "user" feature_names: ["user_id", "age"] wide_deep: DEEP }',
+      '  feature_groups { group_name: "item" feature_names: ["item_id", "cate_id", "price"] wide_deep: DEEP }',
+      '  feature_groups { group_name: "seq" feature_names: ["item_id", "cate_id", "hist_items", "hist_cates"] wide_deep: DEEP }',
+      '  backbone {',
+      '    blocks { name: "user" inputs { feature_group_name: "user" } %s }' % mlp,
+      '    blocks { name: "item" inputs { feature_group_name: "item" } %s }' % mlp,
+      '    blocks { name: "seq_input" inputs { feature_group_name: "seq" } input_layer { output_seq_and_normal_feature: true } }',
+      '    blocks { name: "din" inputs { block_name: "seq_input" } keras_layer { class_name: "DIN" din {',
+      '      attention_dnn { hidden_units: [128, 64, 32, 1] activation: "dice" } need_target_feature: true',
+      '      attention_normalizer: "%s" } } }' % normalizer,
+      '    concat_blocks: ["user", "item", "din"]',
+      '    top_mlp { hidden_units: [256, 128, 64] } }',
+      '  model_params { l2_regularization: 1e-5 }',
+      '  embedding_regularization: 1e-5 }', ''])).encode()
+
+
 def c3_batch(batch_size, seq_len, seed, vocab, cate_buckets=10000, zipf_alpha=1.05):
   """host batch in c3_config_text's InputLayer form: ids feature-major (user_id, age, item_id, cate_id), price,
   histories padded to seq_len with lengths ~ U[1, seq_len], label Bernoulli(0.25).

@@ -527,6 +527,19 @@ int er_din_pool_bwd(const float* probs, const float* keys, const float* gout,
                     const int32_t* lens, int64_t batch, int32_t seq_len, int32_t dim,
                     float* g_scores, float* g_keys, int32_t accumulate_gkeys,
                     er_stream_t stream);
+/* sigmoid pool (attention_normalizer 'sigmoid' of the keras DIN block, layers/keras/din.py:57-60), the
+ * arguments of er_din_pool_* plus `scale` (1/sqrt(history width) there):
+ *   probs[b,t] = t < len ? sigmoid(scale*scores[b,t]) : 0, out[b,:] = sum_t probs[b,t]*keys[b,t,:]
+ *   (ascending t, deterministic);
+ *   bwd: g_scores[b,t] = t < len ? scale*p*(1-p)*(gout[b,:].keys[b,t,:]) : 0,
+ *        g_keys[b,t,:] (+)= p*gout[b,:].  lens NULL: every step counts. */
+int er_din_sigmoid_pool_fwd(const float* scores, const float* keys, const int32_t* lens,
+                            int64_t batch, int32_t seq_len, int32_t dim, float scale,
+                            float* probs, float* out, er_stream_t stream);
+int er_din_sigmoid_pool_bwd(const float* probs, const float* keys, const float* gout,
+                            const int32_t* lens, int64_t batch, int32_t seq_len, int32_t dim,
+                            float scale, float* g_scores, float* g_keys,
+                            int32_t accumulate_gkeys, er_stream_t stream);
 
 /* ---- K5: DCN cross layer (model/dcn.py:32-45): out = x0*(xl.w) + b + xl; xw_out[b] = xl.w.
  * bwd: gxl = gout + w*s, gx0 (+)= gout*xw, gw = sum_b s_b*xl[b,:], gb = sum_b gout[b,:]
