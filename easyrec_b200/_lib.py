@@ -76,6 +76,7 @@ SIGNATURES = {
                              c_vp, c_vp, c_vp]),
     'er_bucketize_weighted': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i32,
                                       c_vp, c_vp, c_vp]),
+    'er_bucketize_seq': (c_i32, [c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp]),
     'er_dropout': (c_i32, [c_vp, c_i64, ctypes.c_float, ctypes.c_uint64, c_vp, c_vp, c_vp]),
     'er_gemm_small_workspace_bytes': (c_sz, [c_i64, c_i64, c_i64]),
     'er_gemm_small': (c_i32, [c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_sz,

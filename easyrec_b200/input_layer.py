@@ -422,25 +422,34 @@ class InputLayer(object):
     self.hyper.set(0.01, 0)
     self.opt_holder = {'opt': self.hyper.opt(embedding_optimizer)}
     # EmbeddingParallel (train_distribute: EmbeddingParallelStrategy): the tables are row-sharded over shard_n ranks
-    # and every single-valued lookup goes through the all-to-all exchange of sharded.ShardedLookup
+    # and every lookup goes through the all-to-all exchange of sharded.ShardedLookup
     self.ep = shard_n > 1
     if self.ep:
       from easyrec_b200.sharded import ShardedLookup
       exchanges = {}   # row plan -> the exchange its arenas share (ids once, rows in one packed all-to-all)
       for dim, subs in self.subcalls.items():
         for sk, sc in subs.items():
-          if sc.kind == 'seq':
-            raise NotImplementedError('EmbeddingParallel with single-valued SequenceFeature slots (DIN histories): those '
-                                      'models run as replicas; id / raw / tag / multi-valued sequence slots are exchanged')
           if sc.kind != 'single':
-            # multi-valued slots (the ragged forms of embedding_parallel_lookup): an exchange of their own.  The owner
-            # applies one row update per exchange, so a table must not be read by slots of two different launches
+            # multi-valued slots (the ragged forms of embedding_parallel_lookup) and un-pooled histories (one lookup per
+            # step, padded steps dropped by K1): an exchange of their own.  The owner applies one row update per
+            # exchange, so a table must not be read by slots of two different launches
             mine = set(slot.table for _, _, slot, _ in sc.items)
             for sk2, sc2 in subs.items():
-              if sc2 is not sc and mine & set(slot.table for _, _, slot, _ in sc2.items):
+              shared = sorted(mine & set(slot.table for _, _, slot, _ in sc2.items)) if sc2 is not sc else None
+              if shared and 'seq' in (sc.kind, sc2.kind):
+                raise NotImplementedError('EmbeddingParallel: table(s) %s are read both by history (SequenceFeature) '
+                                          'steps and by other features; give the histories tables of their own'
+                                          % shared)
+              if shared:
                 raise NotImplementedError('EmbeddingParallel: table(s) %s are shared by single- and multi-valued features'
-                                          % sorted(mine & set(slot.table for _, _, slot, _ in sc2.items)))
-            sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank)
+                                          % shared)
+            if sc.kind == 'seq' and len(subs) > 1 and self.arenas[dim].opt_kind == _lib.OPT_ADAM_ROWS:
+              # adam_optimizer's dense decay sweeps every row the owner did not update: with two exchanges on one arena
+              # each would sweep the rows only the other one updated
+              raise NotImplementedError('EmbeddingParallel: adam_optimizer with histories next to other features of '
+                                        'embedding_dim %d (their tables share one arena and two exchanges)' % dim)
+            seq = (B, sk[1]) if sc.kind == 'seq' else None
+            sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, seq=seq)
             if len(subs) == 1:
               self.merged[dim].sharded = sc.sharded
             continue
@@ -774,6 +783,18 @@ class InputLayer(object):
         rows, w = hit
       outs = E.fused_lookup(call, rows, weights=w)
       return rows, w, None, None, outs
+    if sc.kind == 'seq' and self.ep:
+      # row-sharded tables: er_bucketize_seq (owner, local row; -1 on padded steps) -> K8 -> all-to-alls -> every
+      # received row written to its own step's row of the [B*T, sum D] matrix
+      T = sc.n_seg_per_slot // B
+      seqs = [features['seq_fea'][fname] for _, fname, _, _ in sc.items]
+      ids = torch.cat([i.reshape(-1) for i, _ in seqs]) if len(seqs) > 1 else seqs[0][0].reshape(-1)
+      lens = torch.cat([n.reshape(-1) for _, n in seqs]) if len(seqs) > 1 else seqs[0][1].reshape(-1)
+      outs = call.alloc_outputs()
+      rows = sc.sharded.forward(ids.contiguous(), None, outs, lens=lens.to(torch.int32).contiguous())
+      for o in outs:
+        o.requires_grad_(True)
+      return rows, None, None, None, outs
     if sc.kind == 'seq':
       T = sc.n_seg_per_slot // B
       ids_list, pad_list = [], []

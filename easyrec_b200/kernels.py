@@ -121,6 +121,25 @@ def bucketize(ids, slots_dev, n_slots, n_seg, seg_ids=None, row_ptr=None, rows=N
   return rows
 
 
+def bucketize_seq(ids, lens, batch, seq_len, slots_dev, n_slots, rows=None, owner=None):
+  """K1 over un-pooled histories (er_bucketize_seq): ids int64 [n_features * batch * seq_len] steps, lens int32
+  [n_features * batch].  Steps at or beyond their sample's length come out as rows = owner = -1."""
+  lib = _lib.load()
+  _chk(ids, torch.int64, 'ids')
+  _chk(lens, torch.int32, 'lens')
+  _chk(owner, torch.int32, 'owner')
+  n_features = lens.numel() // batch
+  assert lens.numel() == n_features * batch and ids.numel() == lens.numel() * seq_len
+  if rows is None:
+    rows = torch.empty_like(ids)
+  _chk(rows, torch.int64, 'rows')
+  assert rows.numel() == ids.numel() and (owner is None or owner.numel() == ids.numel())
+  _lib.check(
+      lib.er_bucketize_seq(_p(ids), _p(lens), int(batch), int(seq_len), n_features, _p(slots_dev), n_slots, _p(rows),
+                           _p(owner), _stream()), 'er_bucketize_seq')
+  return rows
+
+
 def k1_weight_args(ids, weights):
   """Keyword arguments of bucketize() that hand a weighted CSR call's lookup weights to K1, so that the lookups the
   pooling prunes are dropped before K7, er_mark_rows and K8 see them.  Only device tensors take this path: the host

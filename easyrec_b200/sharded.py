@@ -106,9 +106,10 @@ class ShardedExchange(object):
     if self._pre is not None:
       torch.cuda.current_stream().wait_stream(self._pre)
 
-  def lookup(self, first, ids, seg_ids=None, row_ptr=None, weights=None):
+  def lookup(self, first, ids, seg_ids=None, row_ptr=None, weights=None, lens=None):
     """K1 -> K8 -> all_to_all(ids) -> every member's K2 on the owner -> ONE all_to_all(rows).  weights: the lookup
-    weights of a CSR call (K1 drops the mean / sqrtn lookups they prune, so K8 does not request those rows)."""
+    weights of a CSR call (K1 drops the mean / sqrtn lookups they prune, so K8 does not request those rows).  lens:
+    the history lengths of an un-pooled sequence call (er_bucketize_seq: padded steps request nothing)."""
     N = self.world
     call = first.call
     if seg_ids is not None:
@@ -126,8 +127,12 @@ class ShardedExchange(object):
       self.rows_local.copy_(self.rows_local_n)
       self._have_next = False
     else:
-      K.bucketize(ids, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr, rows=self.rows_local,
-                  owner=self.owner, **K.k1_weight_args(ids, weights))
+      if lens is not None:
+        K.bucketize_seq(ids, lens, first.seq[0], first.seq[1], call.slots_dev, call.n_slots, rows=self.rows_local,
+                        owner=self.owner)
+      else:
+        K.bucketize(ids, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr,
+                    rows=self.rows_local, owner=self.owner, **K.k1_weight_args(ids, weights))
       K.shard_group(self.rows_local, self.owner, N, self.cap, self.send_rows, self.pos, self.counts, self.group_ws)
       self.overflow += self.counts[N:]
       dist.all_to_all_single(self.recv_rows, self.send_rows)
@@ -183,9 +188,12 @@ class ShardedLookup(object):
   gathers a zero row and its gradient slot is dropped by K7), so nothing is read back on the host and the exchange
   is captured in the step's CUDA graph with the rest.  A block that overflows loses lookups: counted on the device,
   raised by check().  Arenas with the same row plan share one ShardedExchange: ids travel once and the rows of all of
-  them in one packed all-to-all per direction.  Single-valued slots (the packed sparse_fea / raw projections)."""
+  them in one packed all-to-all per direction.  Single-valued slots (the packed sparse_fea / raw projections), the
+  ragged (CSR) slots, and un-pooled histories: `seq = (batch, seq_len)` makes every step of the call one lookup and one
+  segment, K1 is er_bucketize_seq (padded steps ask for no row) and the pooling K2 writes each received row to its own
+  step's row of the call's [batch * seq_len, sum D] matrix."""
 
-  def __init__(self, call, world, rank, exchange=None, slack=None):
+  def __init__(self, call, world, rank, exchange=None, slack=None, seq=None):
     a = call.arena
     assert a.shard_n == world and a.shard_rank == rank
     self.call, self.world, self.rank = call, world, rank
@@ -193,6 +201,8 @@ class ShardedLookup(object):
     # slots - TagFeatures, multi-valued sequence steps (the ragged forms of embedding_parallel_lookup,
     # feature_column.py:248-357 `ragged_ids / ragged_lens`)
     self.csr = not call.single_valued
+    self.seq = seq
+    assert seq is None or (not self.csr and exchange is None)
     self.L = L = call.max_lookups
     slack = float(os.environ.get('ER_EP_SLACK', '1.25')) if slack is None else slack
     # distinct rows this rank can ask one peer for: every lookup of the hashed / identity slots in the worst case
@@ -228,15 +238,16 @@ class ShardedLookup(object):
     self.recv_view = ex.recv_emb[:, self.col:self.col + D]   # this arena's received rows: the pooling K2's "table"
     self.sum_view = ex.send_g[:, self.col:self.col + D]      # ... and the requester-side gradient sums
 
-  def forward(self, ids, weights, outs, row_ptr=None, seg_ids=None):
+  def forward(self, ids, weights, outs, row_ptr=None, seg_ids=None, lens=None):
     """ids int64 [L] in the call's slot order (None for a member whose exchange already ran this step); writes the
     pooled rows into `outs` (the call's output matrices).  Multi-valued slots: ids padded to the lookup capacity,
-    row_ptr int32 [n_seg + 1] and seg_ids int32 [L] of the CSR (lookups beyond row_ptr[-1] are ignored)."""
+    row_ptr int32 [n_seg + 1] and seg_ids int32 [L] of the CSR (lookups beyond row_ptr[-1] are ignored).  Histories:
+    ids [n_features * batch * seq_len] steps and lens int32 [n_features * batch]."""
     ex, call = self.ex, self.call
     ex.build()
-    assert (row_ptr is not None) == self.csr
+    assert (row_ptr is not None) == self.csr and (lens is not None) == (self.seq is not None)
     if ids is not None:
-      ex.lookup(self, ids, seg_ids=seg_ids, row_ptr=row_ptr, weights=weights if self.csr else None)
+      ex.lookup(self, ids, seg_ids=seg_ids, row_ptr=row_ptr, weights=weights if self.csr else None, lens=lens)
     K.embedding_fwd(self.recv_view, call.arena.dim, ex.pos, self.pool_slots, call.n_slots, call.n_seg, outs, weights=weights,
                     row_ptr=row_ptr, seg_scale=call.seg_scale)
     self._weights = weights

@@ -172,6 +172,20 @@ int er_bucketize_weighted(const int64_t* ids, const float* weights, const int32_
                           const er_slot_t* slots, int32_t n_slots, int64_t* rows,
                           int32_t* owner, er_stream_t stream);
 
+/* er_bucketize over un-pooled histories (SequenceFeature slots without a
+ * combiner): ids and rows are [n_features, batch, seq_len] steps, step
+ * l = (f*batch + b)*seq_len + t is segment l of the slot plan, and
+ * lens[f*batch + b] is the length of that sample's history.  A step with
+ * t >= lens[...] is padding: rows[l] = owner[l] = -1 and its id is not read,
+ * so K8 never requests it.  A length below 0 pads every step and one above
+ * seq_len pads none (lengths are clamped to [0, seq_len]).  Live steps follow
+ * er_bucketize bit for bit (rows, owner and dropped ids).  One launch,
+ * deterministic, no allocation; n_features*batch*seq_len < 2^31. */
+int er_bucketize_seq(const int64_t* ids, const int32_t* lens, int64_t batch,
+                     int32_t seq_len, int32_t n_features, const er_slot_t* slots,
+                     int32_t n_slots, int64_t* rows, int32_t* owner,
+                     er_stream_t stream);
+
 /* ---- K8: index bucketing of the row-sharded lookup --------------------
  * Replaces the Unique + dynamic_partition + host-read split sizes of
  * embedding_parallel_lookup (compat/feature_column/feature_column.py:258-303).
