@@ -1730,6 +1730,9 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
       return fail(ER_ERR_WORKSPACE, "er_embedding_bwd_reuse_sort: source workspace too small");
     if (!bucketed)
       return fail(ER_ERR_UNSUPPORTED, "er_embedding_bwd_reuse_sort: uniq_rows output needs the rows (er_embedding_bwd)");
+    if (k7_warp_mode(sorted_dim) != k7_warp_mode(dim))
+      return fail(ER_ERR_UNSUPPORTED, "er_embedding_bwd_reuse_sort: the placement was made in the other placement mode "
+                                      "(warp-sized buckets for dims 1, 4, 8, 16 and 32, CTA-sized for the others)");
     src = bwd_carve(const_cast<void*>(sorted_ws), n_lookups_cap, sorted_dim);
     cudaMemsetAsync(w.counters, 0, bk::zero_call_bytes(), st);
   } else if (bucketed) {
@@ -1737,11 +1740,7 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
   } else {
     rsort::sort_rows(rows, n_lookups_cap, n_dev, n_rows, w.keys, w.vals, w.sort_ws, w.counters, st);
   }
-  // the mode the placement was made in: a table that reuses another table's placement follows it
-  const bool place_warp = k7_warp_mode(sorted_ws ? sorted_dim : dim);
-  if (bucketed && place_warp && !k7_warp_mode(dim))
-    return fail(ER_ERR_UNSUPPORTED, "er_embedding_bwd_reuse_sort: the placement was made for warp-sized buckets, "
-                                    "rows of this dim need CTA-sized ones (presort with this dim instead)");
+  const bool place_warp = k7_warp_mode(dim);
 
   BwdArgs a = {};
   a.table = table;

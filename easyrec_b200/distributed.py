@@ -95,6 +95,7 @@ class DataParallel(object):
     self.input_layer = input_layer
     self.world = world
     self.sparse = sparse
+    self.placements = E.Placements()   # K7 placements over the gathered rows
     if not sparse:
       self.dense_opt = dense_opt
       dense_opt.grad_scale = 1.0 / world
@@ -119,12 +120,12 @@ class DataParallel(object):
     """At the head of the step: K1 on this rank's batch, all-gather of the rows and per-lookup weights, and the
     global dedup sort started on a side stream - it needs no gradient, so it runs under the dense forward/backward
     (with N ranks it is N times the single-GPU sort)."""
+    self.placements.clear()
     if not self.prephase:
       return
     il = self.input_layer
     self._pre = {}
     owners = {}
-    todo = []
     plans = il.precompute_rows(features)   # K1 on the step's stream
     if self._side is None and plans:
       self._side = torch.cuda.Stream(device=plans[0][2].device)
@@ -136,17 +137,15 @@ class DataParallel(object):
       for dim, m, rows, w in plans:
         g = self.gcalls[id(m)]
         first = owners.get(id(rows))
-        if first is not None and first.call.arena.n_rows == m.arena.n_rows:
-          self._pre[id(m)] = (first, False)
-          continue
-        owners[id(rows)] = g
-        dist.all_gather_into_tensor(g.rows, self._rows_to_send(g, rows))
-        if w is not None:
-          dist.all_gather_into_tensor(g.weights, w)
-        self._pre[id(m)] = (g, True)
-        todo.append(g)
-      for g in todo:
-        K.embedding_bwd_presort(g.rows, g.call.arena.n_rows, g.call.arena.dim, g.ws, g.slots_dev, g.n_slots)
+        if first is None or first.call.arena.n_rows != m.arena.n_rows:
+          first = owners[id(rows)] = g
+          dist.all_gather_into_tensor(g.rows, self._rows_to_send(g, rows))
+          if w is not None:
+            dist.all_gather_into_tensor(g.weights, w)
+        self._pre[id(m)] = first
+      for dim, m, rows, w in plans:
+        g = self.gcalls[id(m)]
+        self.placements.presort(self._pre[id(m)].rows, m.arena.n_rows, dim, g.ws, g.slots_dev, g.n_slots)
 
   def sync_dense_grads(self):
     """sum over replicas in one bucket; the 1/world of hvd.allreduce(Average)
@@ -161,14 +160,11 @@ class DataParallel(object):
       # (lookups past a rank's real count carry row -1 and are dropped by K7 whatever segment they name)
       dist.all_gather_into_tensor(g.seg_ids, seg_ids.contiguous())
       g.seg_ids.add_(g.seg_off)
-    pre = self._pre.get(id(call))
-    if pre is not None:   # rows / weights were gathered (and their sort started) before the step
-      owner, is_owner = pre
-      g.rows_src = None if is_owner else owner
-      g.presorted = True
+    owner = self._pre.get(id(call))
+    if owner is not None:   # rows / weights were gathered (and their sort started) before the step
+      g.rows_src = None if owner is g else owner
       self._gather_grads(g, call, outs, w)
       return g
-    g.presorted = False
     # arenas with the same row plan (wide dim-1 next to the deep tables) were looked up with the SAME rows /
     # weights tensors: gather those once and let the later call alias the first one's buffers (and its sort)
     first = self._rows_owner.get(id(rows))
@@ -246,14 +242,11 @@ class DataParallel(object):
     for call, rows, w, outs, seg_ids in pending:
       g = self.gcalls[id(call)]
       a = call.arena
-      src = getattr(g, 'rows_src', None)
-      owner = src if src is not None else g
-      sorted_from = None
-      if src is not None or getattr(g, 'presorted', False):
-        sorted_from = (owner.ws, owner.call.arena.dim)
+      owner = getattr(g, 'rows_src', None) or g   # the GlobalCall whose buffers hold the gathered rows / weights
       K.embedding_bwd(a.weight, a.state0, a.state1, a.dim, owner.rows, g.slots_dev, g.n_slots, g.n_seg,
                       g.grads, opt, g.ws, weights=owner.weights if w is not None else None,
-                      seg_ids=g.seg_ids if seg_ids is not None else None, seg_scale=g.seg_scale, sorted_from=sorted_from)
+                      seg_ids=g.seg_ids if seg_ids is not None else None, seg_scale=g.seg_scale,
+                      sorted_from=self.placements.sorted_from(owner.rows, a.n_rows, a.dim, g.ws))
       if g.one_row:
         K.sparse_apply(a.weight, a.state0, a.state1, a.dim, g.one_row_rows, g.one_row_sums, None, opt)
       # tf.train.AdamOptimizer: the rows nobody looked up decay too

@@ -214,6 +214,36 @@ def fused_backward_update(call, rows, outs, opt, weights=None, row_ptr=None, seg
   adam_dense_decay(a, rows, opt, n_dev=None if row_ptr is None else row_ptr[call.n_seg:])
 
 
+class Placements(object):
+  """K7's bucket placements shared by the updates of one step: one per (rows tensor, n_rows, placement mode).  Tables
+  looked up with the same rows (the wide dim-1 table next to the deep ones) whose dims share a mode - warp-sized or
+  CTA-sized buckets, K.k7_warp_mode - need the same placement, so reusing it (er_embedding_bwd_reuse_sort) only skips
+  work and never changes a result.  clear() at the start of every step; `presorted`: presort() launched work that the
+  updates' stream has to join."""
+
+  def __init__(self):
+    self.clear()
+
+  def presort(self, rows, n_rows, dim, ws, slots_dev, n_slots, seg_ids=None):
+    """place the key's lookups into `ws` now, on the current stream, unless the key has a placement"""
+    if self.sorted_from(rows, n_rows, dim, ws) is None:
+      K.embedding_bwd_presort(rows, n_rows, dim, ws, slots_dev, n_slots, seg_ids=seg_ids)
+      self.presorted = True
+
+  def sorted_from(self, rows, n_rows, dim, ws):
+    """embedding_bwd's sorted_from: the key's placement (ws, dim), or None when this update into `ws` is the first of
+    its key - it places itself and later updates of the key reuse its placement."""
+    key = (id(rows), int(n_rows), K.k7_warp_mode(dim))
+    hit = self._placed.get(key)
+    if hit is None:
+      self._placed[key] = (ws, dim)
+    return hit
+
+  def clear(self):
+    self._placed = {}
+    self.presorted = False
+
+
 class _FM(torch.autograd.Function):
   """K3: layers/fm.py:20-26 on the [B, F*D] group matrix."""
 

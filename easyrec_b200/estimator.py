@@ -194,7 +194,6 @@ class EasyRecEstimator(object):
     self.input_layer.drop_prefetch()   # (an id exchange prefetched for the next TRAINING batch is not this batch's)
     logits = self.model(feats)
     self.input_layer._pending = []
-    self.input_layer._presorted = {}
     return logits
 
   def _group_fields(self):

@@ -465,7 +465,7 @@ class InputLayer(object):
     self.replica_grad_scale = getattr(self, '_ep_scale', 1.0)
     self._pending = []
     self._rows_cache = {}
-    self._presorted = {}
+    self.placements = E.Placements()
     self._side = None
     self.presort_enabled = True
     self._preset_rows = {}
@@ -494,19 +494,14 @@ class InputLayer(object):
         m.sharded.backward_update(outs, self.opt_holder['opt'])
       self._pending = []
       return
-    sorted_by = dict(self._presorted)   # id(rows tensor) -> (workspace, dim, n_rows) of the call that sorted it
-    if self._presorted:
+    if self.placements.presorted:
       torch.cuda.current_stream().wait_stream(self._side)   # join the early sorts
-      self._presorted = {}
     cur = torch.cuda.current_stream() if str(self.device).startswith('cuda') else None
     forked = False
     for idx, (m, rows, w, outs, seg_ids) in enumerate(self._pending):
       # arenas with the same row plan (DeepFM / Wide&Deep: the wide dim-1 and the deep tables) look up the
-      # same rows tensor: the second K7 reuses the first one's bucket placement.
-      hit = sorted_by.get(id(rows))
-      # (a placement made for warp-sized buckets serves only tables whose rows a warp can stage)
-      src = (hit[0], hit[1]) if (hit is not None and hit[2] == m.arena.n_rows and
-                                 (not K.k7_warp_mode(hit[1]) or K.k7_warp_mode(m.arena.dim))) else None
+      # same rows tensor: a later K7 may reuse an earlier one's bucket placement.
+      src = self.placements.sorted_from(rows, m.arena.n_rows, m.arena.dim, m.ws)
       if idx > 0 and src is not None and self._side is not None and cur is not None:
         # different arenas, sort already done: this update runs beside the first one on the side stream
         if not forked:
@@ -516,8 +511,6 @@ class InputLayer(object):
           E.fused_backward_update(m, rows, outs, self.opt_holder['opt'], weights=w, seg_ids=seg_ids, sorted_from=src)
       else:
         E.fused_backward_update(m, rows, outs, self.opt_holder['opt'], weights=w, seg_ids=seg_ids, sorted_from=src)
-      if hit is None:
-        sorted_by[id(rows)] = (m.ws, m.arena.dim, m.arena.n_rows)
     if forked:
       cur.wait_stream(self._side)
     self._pending = []
@@ -610,11 +603,7 @@ class InputLayer(object):
         if sc.kind != 'single' or len(subs) != 1:
           continue
         call = sc.call
-        key = getattr(sc, 'rows_key', None)
-        if key is None:
-          key = (tuple((int(r['num_buckets']), int(r['row_offset']), int(r['seg_begin']), int(r['n_seg']),
-                        int(r['bucket_mode']), int(r['shard_n'])) for r in call.slots_np), tuple(call.sources))
-          sc.rows_key = key
+        key = self._rows_key(sc)
         hit = self._preset_rows.get(key)
         if hit is None:
           cids, w = self._gather_inputs(dim, features.get('sparse_fea'), dense_norm)
@@ -627,22 +616,16 @@ class InputLayer(object):
   def _presort(self):
     """K7's bucket placement needs only the looked-up rows: start it now on a side stream so it runs under the
     dense forward/backward instead of after it (joined in backward_update; captured as a fork/join)."""
-    self._presorted = {}
-    if not (self.presort_enabled and not self.ep and torch.is_grad_enabled() and str(self.device).startswith('cuda')):
-      return
-    todo = []
-    for m, rows, w, outs, seg_ids in self._pending:
-      if id(rows) not in self._presorted:
-        self._presorted[id(rows)] = (m.ws, m.arena.dim, m.arena.n_rows)
-        todo.append((m, rows, seg_ids))
-    if not todo:
+    self.placements.clear()
+    if not (self._pending and self.presort_enabled and not self.ep and torch.is_grad_enabled() and
+            str(self.device).startswith('cuda')):
       return
     if self._side is None:
       self._side = torch.cuda.Stream(device=self.device)
     self._side.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(self._side):
-      for m, rows, sids in todo:
-        K.embedding_bwd_presort(rows, m.arena.n_rows, m.arena.dim, m.ws, m.slots_dev, m.n_slots, seg_ids=sids)
+      for m, rows, w, outs, seg_ids in self._pending:
+        self.placements.presort(rows, m.arena.n_rows, m.arena.dim, m.ws, m.slots_dev, m.n_slots, seg_ids=seg_ids)
 
   def normalize_dense(self, dense):
     if self.raw_has_range:

@@ -309,8 +309,8 @@ class StepHyper(object):
 def embedding_bwd(table, state0, state1, dim, rows, slots_dev, n_slots, n_seg, grad_bufs, opt,
                   ws, weights=None, seg_ids=None, row_ptr=None, seg_scale=None, row_stride=None,
                   uniq_rows=None, uniq_grads=None, n_uniq=None, n_rows=None, sorted_from=None):
-  """sorted_from = (ws, dim) of an earlier embedding_bwd on this stream over the SAME rows tensor and a
-  table with the same n_rows: its bucket placement is reused (er_embedding_bwd_reuse_sort)."""
+  """sorted_from = (ws, dim) of an earlier embedding_bwd on this stream over the SAME rows tensor, n_rows and placement
+  mode (k7_warp_mode): its bucket placement is reused (er_embedding_bwd_reuse_sort)."""
   lib = _lib.load()
   row_stride = dim
   if table is not None:

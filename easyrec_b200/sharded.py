@@ -35,7 +35,7 @@ class ShardedExchange(object):
     self._summed = 0        # members whose requester-side gradient sums are in send_g
     self._side = torch.cuda.Stream(device=device) if str(device).startswith('cuda') else None
     self._pre = torch.cuda.Stream(device=device) if str(device).startswith('cuda') else None
-    self._presorted = False
+    self.placements = E.Placements()   # the members' K7 placements, requester and owner side
     self._have_next = False   # K1 / K8 / id all-to-all of the NEXT batch already sit in the *_n buffers
     # global-norm clipping: the owners hold their row update after the gradient exchange until the norm of every
     # rank's received gradients is known (ShardedLookup.apply_held)
@@ -136,27 +136,20 @@ class ShardedExchange(object):
       K.shard_group(self.rows_local, self.owner, N, self.cap, self.send_rows, self.pos, self.counts, self.group_ws)
       self.overflow += self.counts[N:]
       dist.all_to_all_single(self.recv_rows, self.send_rows)
-    self._presorted = False
+    self.placements.clear()
     if self._side is not None and torch.is_grad_enabled() and seg_ids is None:
       # the row-only halves of both K7s (requester: positions, owner: received rows) need no gradient: a parallel
       # branch under the row exchange and the dense forward / backward, joined in the backward
-      m = max(self.members, key=lambda x: x.call.arena.dim)   # (a placement for wide rows serves the narrow tables too)
       self._side.wait_stream(torch.cuda.current_stream())
       with torch.cuda.stream(self._side):
-        K.embedding_bwd_presort(self.pos, self.n_ex, m.call.arena.dim, m.pool_ws, m.pool_slots, m.call.n_slots)
-        K.embedding_bwd_presort(self.recv_rows, m.call.arena.n_rows, m.call.arena.dim, m.owner_ws, m.owner_slots, 1)
-      self._presorted = m
+        for m in self.members:
+          a = m.call.arena
+          self.placements.presort(self.pos, self.n_ex, a.dim, m.pool_ws, m.pool_slots, m.call.n_slots)
+          self.placements.presort(self.recv_rows, a.n_rows, a.dim, m.owner_ws, m.owner_slots, 1)
     for m in self.members:
       K.embedding_fwd(m.call.arena.weight, m.call.arena.dim, self.recv_rows, m.owner_slots, 1, self.n_ex, [self.send_emb])
     dist.all_to_all_single(self.recv_emb, self.send_emb)
     self._active, self._summed = [], 0
-
-  def sorted_from(self, member, which):
-    """(workspace, dim) of the early placement a member's K7 may reuse, or None."""
-    m = self._presorted
-    if not m or not (K.k7_warp_mode(member.call.arena.dim) or not K.k7_warp_mode(m.call.arena.dim)):
-      return None
-    return (m.pool_ws if which == 'pool' else m.owner_ws, m.call.arena.dim)
 
   def check(self):
     bad = int(self.mismatch.item())
@@ -265,12 +258,12 @@ class ShardedLookup(object):
       for g in gbufs:   # (the trainer runs this backward on a side stream: the gradients were produced on the main one)
         g.record_stream(torch.cuda.current_stream())
     if ex._summed == 0:
-      if ex._presorted:
+      if ex.placements.presorted:
         torch.cuda.current_stream().wait_stream(ex._side)
       ex.send_g.zero_()
     K.embedding_bwd(self.sum_view, None, None, D, ex.pos, self.pool_slots, call.n_slots, call.n_seg, gbufs, self.sum_opt,
                     self.pool_ws, weights=self._weights, seg_ids=getattr(self, '_seg_ids', None), seg_scale=call.seg_scale,
-                    n_rows=self.n_ex, sorted_from=ex.sorted_from(self, 'pool'))
+                    n_rows=self.n_ex, sorted_from=ex.placements.sorted_from(ex.pos, self.n_ex, D, self.pool_ws))
     ex._summed += 1
     if ex._summed < len(ex._active):
       return
@@ -295,7 +288,8 @@ class ShardedLookup(object):
     for m in ex._active:
       a = m.call.arena
       K.embedding_bwd(a.weight, a.state0, a.state1, a.dim, ex.recv_rows, m.owner_slots, 1, m.n_ex, [ex.recv_g], opt,
-                      m.owner_ws, n_rows=a.n_rows, sorted_from=ex.sorted_from(m, 'owner'))
+                      m.owner_ws, n_rows=a.n_rows,
+                      sorted_from=ex.placements.sorted_from(ex.recv_rows, a.n_rows, a.dim, m.owner_ws))
       E.adam_dense_decay(a, ex.recv_rows, opt)
     if struct_scaled:
       opt.grad_scale = opt.grad_scale * N

@@ -283,7 +283,11 @@ int er_embedding_bwd_presort(const int64_t* rows, int64_t n_rows, const int32_t*
  * next to the deep table of DeepFM / Wide&Deep) was already prepared by er_embedding_bwd_presort or
  * deduplicated by an earlier er_embedding_bwd on this stream whose workspace is sorted_ws (allocated for
  * dimension sorted_dim and left untouched since): only the per-row sums and the row updates run.  `ws` is this
- * call's own workspace (er_embedding_bwd_workspace_bytes(n, dim)).  uniq_rows output is not available here. */
+ * call's own workspace (er_embedding_bwd_workspace_bytes(n, dim)).  uniq_rows output is not available here.
+ * Precondition: dim and sorted_dim are in the same placement mode - both in {1, 4, 8, 16, 32} (warp-sized buckets)
+ * or both outside it (CTA-sized buckets).  The reused placement is then the one this call would have made, so the
+ * result equals er_embedding_bwd's bit for bit.  A placement of the other mode returns ER_ERR_UNSUPPORTED before
+ * anything is written. */
 int er_embedding_bwd_reuse_sort(float* table, float* state0, float* state1, int64_t n_rows,
                                 int32_t dim, int32_t row_stride, const int64_t* rows,
                                 const float* weights, const int32_t* seg_ids,

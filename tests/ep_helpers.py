@@ -62,12 +62,14 @@ def compare(dp_il, ep_il, rank, world, atol):
   return worst
 
 
-def run(make_estimator, dev, rank, world, steps=4, atol=2e-6, lookahead=False):
-  """make_estimator(config bytes, embedding_parallel) -> EasyRecEstimator on `dev`"""
-  dp = make_estimator(CFG_EP.replace(b'train_distribute: EmbeddingParallelStrategy', b''), False)
-  ep = make_estimator(CFG_EP, None)
+def run(make_estimator, dev, rank, world, steps=4, atol=2e-6, lookahead=False, cfg=CFG_EP):
+  """make_estimator(config bytes, embedding_parallel) -> EasyRecEstimator on `dev`; cfg: a row-sharded config over
+  the inputs of batch()"""
+  dp = make_estimator(cfg.replace(b'train_distribute: EmbeddingParallelStrategy', b''), False)
+  ep = make_estimator(cfg, None)
   assert ep.embedding_parallel and not dp.embedding_parallel and ep.input_layer.ep
-  assert ep.input_layer.arenas[8].n_rows < dp.input_layer.arenas[8].n_rows      # (V + N - 1) // N rows per table
+  for dim, a in dp.input_layer.arenas.items():
+    assert ep.input_layer.arenas[dim].n_rows < a.n_rows      # (V + N - 1) // N rows per table
   copy_tables(dp.input_layer, ep.input_layer, rank, world)
   ep.model.load_state_dict(dp.model.state_dict())
   ep.trainer.dense_opt.flat_p.copy_(dp.trainer.dense_opt.flat_p)

@@ -5,7 +5,7 @@ spawned worker processes."""
 import numpy as np
 import torch
 
-from easyrec_b200 import kernels as K, trainer as T
+from easyrec_b200 import _lib, kernels as K, trainer as T
 from oracle import oracle as O
 
 
@@ -79,6 +79,10 @@ def install_sparse(patch):
   def embedding_bwd(table, state0, state1, dim, rows, slots_dev, n_slots, n_seg, grad_bufs, opt, ws, weights=None,
                     seg_ids=None, row_ptr=None, seg_scale=None, row_stride=None, uniq_rows=None, uniq_grads=None,
                     n_uniq=None, n_rows=None, sorted_from=None):
+    if sorted_from is not None and K.k7_warp_mode(sorted_from[1]) != K.k7_warp_mode(dim):
+      # er_embedding_bwd_reuse_sort's precondition: a placement is reused only by a table of its own placement mode
+      raise _lib.ErError('er_embedding_bwd_reuse_sort: a dim-%d placement reused by a dim-%d table (other placement '
+                         'mode)' % (sorted_from[1], dim))
     sl = _slots(slots_dev)
     gseg = np.zeros((n_seg, dim), np.float32)
     for s in sl:

@@ -153,39 +153,75 @@ def test_clustered_rows_and_device_side_counts():
   _check(got, want, long_rows=list(np.flatnonzero(runs > 32)))
 
 
-def test_presort_then_two_tables_equals_fresh_calls():
-  """DeepFM's plan: the wide dim-1 table reuses the placement of the deep dim-16 call."""
+def _reuse_case(V, B, F, dim):
+  r2 = np.random.default_rng(dim)
+  table = t(r2.normal(size=(V, dim)).astype(np.float32))
+  acc = t(np.full((V, dim), 0.1, np.float32))
+  stride = (F * dim + 3) // 4 * 4
+  gout = t(r2.normal(size=(B, stride)).astype(np.float32))
+  recs = [dict(num_buckets=V, row_offset=0, seg_begin=f * B, n_seg=B, bucket_mode=3, combiner=0, out_buf=0,
+               out_stride=stride, out_col=f * dim) for f in range(F)]
+  return table, acc, gout, K.slots_to_device(K.make_slots(recs), DEV)
+
+
+def _reuse_rows(V, B, F):
   rng = np.random.default_rng(21)
-  V, B, F = 3000, 400, 5
   rows = (rng.zipf(1.2, B * F) % V).astype(np.int64)
   rows[rng.integers(0, B * F, 30)] = -1
   rows[rng.integers(0, B * F, 200)] = 7
-  d_rows = t(rows)
+  return t(rows)
+
+
+def _presort_then_two_tables_equals_fresh_calls(first, second):
+  """the second table reuses the placement of the first call, of the same placement mode: bit for bit a fresh call"""
+  V, B, F = 3000, 400, 5
+  d_rows = _reuse_rows(V, B, F)
   res = {}
   for mode in ('fresh', 'reuse'):
     out = []
-    ws16 = K.bwd_workspace(B * F, DEV, 16)
-    for dim in (16, 1):
-      r2 = np.random.default_rng(dim)
-      table = t(r2.normal(size=(V, dim)).astype(np.float32))
-      acc = t(np.full((V, dim), 0.1, np.float32))
-      stride = (F * dim + 3) // 4 * 4
-      gout = t(r2.normal(size=(B, stride)).astype(np.float32))
-      recs = [dict(num_buckets=V, row_offset=0, seg_begin=f * B, n_seg=B, bucket_mode=3, combiner=0, out_buf=0,
-                   out_stride=stride, out_col=f * dim) for f in range(F)]
-      sd = K.slots_to_device(K.make_slots(recs), DEV)
-      ws = ws16 if dim == 16 else K.bwd_workspace(B * F, DEV, dim)
+    ws_first = K.bwd_workspace(B * F, DEV, first)
+    for dim in (first, second):
+      table, acc, gout, sd = _reuse_case(V, B, F, dim)
+      ws = ws_first if dim == first else K.bwd_workspace(B * F, DEV, dim)
       src = None
       if mode == 'reuse':
-        if dim == 16:
-          K.embedding_bwd_presort(d_rows, V, 16, ws16, sd, F)
-        src = (ws16, 16)
+        if dim == first:
+          K.embedding_bwd_presort(d_rows, V, first, ws_first, sd, F)
+        src = (ws_first, first)
       K.embedding_bwd(table, acc, None, dim, d_rows, sd, F, B * F, [gout], K.make_opt(_lib.OPT_ADAGRAD, 0.05), ws,
                       sorted_from=src)
       out.append((table.cpu(), acc.cpu()))
     res[mode] = out
   for (ta, aa), (tb, ab) in zip(res['fresh'], res['reuse']):
     assert torch.equal(ta, tb) and torch.equal(aa, ab)
+
+
+def test_presort_then_two_tables_equals_fresh_calls():
+  """DeepFM's plan: the wide dim-1 table reuses the placement of the deep dim-16 call (warp-sized buckets)."""
+  _presort_then_two_tables_equals_fresh_calls(16, 1)
+
+
+def test_presort_then_two_cta_mode_tables_equals_fresh_calls():
+  """the same with CTA-sized buckets: a dim-10 table reuses the placement of a dim-64 call."""
+  _presort_then_two_tables_equals_fresh_calls(64, 10)
+
+
+@pytest.mark.parametrize('placed,dim', [(16, 64), (64, 16)])
+def test_reuse_across_placement_modes_is_refused(placed, dim):
+  """A warp-mode placement is no placement for a CTA-mode table, nor the other way round: ER_ERR_UNSUPPORTED, and
+  neither the table nor its optimizer state moves."""
+  V, B, F = 3000, 400, 5
+  d_rows = _reuse_rows(V, B, F)
+  _, _, _, sd_placed = _reuse_case(V, B, F, placed)
+  ws_placed = K.bwd_workspace(B * F, DEV, placed)
+  K.embedding_bwd_presort(d_rows, V, placed, ws_placed, sd_placed, F)
+  table, acc, gout, sd = _reuse_case(V, B, F, dim)
+  table0, acc0 = table.clone(), acc.clone()
+  with pytest.raises(_lib.ErError, match=r'\(status %d\)' % _lib.ER_ERR_UNSUPPORTED):
+    K.embedding_bwd(table, acc, None, dim, d_rows, sd, F, B * F, [gout], K.make_opt(_lib.OPT_ADAGRAD, 0.05),
+                    K.bwd_workspace(B * F, DEV, dim), sorted_from=(ws_placed, placed))
+  torch.cuda.synchronize()
+  assert torch.equal(table, table0) and torch.equal(acc, acc0)
 
 
 def test_c2_size_bucketed_equals_radix_engine_and_is_deterministic():
