@@ -545,9 +545,8 @@ class Backbone(nn.Module):
     def groups(name, as_list=False):
       if build:
         if as_list:
-          return [torch.empty(batch_size, e[2], device='meta') for e in il.group_layout[name]]
-        width = sum(e[2] for e in il.group_layout[name])
-        return torch.empty(batch_size, width, device='meta')
+          return [torch.empty(batch_size, e.width, device='meta') for e in il.group_layout[name]]
+        return torch.empty(batch_size, il.group_width(name), device='meta')
       return list(group_tensors[name][1]) if as_list else group_tensors[name][0]
 
     def seq_group(name):
@@ -555,10 +554,9 @@ class Backbone(nn.Module):
       # lengths of the first sequence feature, plain features concatenated or None)
       if build:
         sl = il.seq_group_layout[name]
-        tw = sum(e[2] for e in il.group_layout[name])
-        return (torch.empty(batch_size, sl['T'], sum(e[1] for e in sl['seq']), device='meta'),
+        return (torch.empty(batch_size, sl['T'], sum(e.dim for e in sl['seq']), device='meta'),
                 torch.empty(batch_size, dtype=torch.int32, device='meta'),
-                torch.empty(batch_size, tw, device='meta') if il.group_layout[name] else None)
+                torch.empty(batch_size, il.group_width(name), device='meta') if il.group_layout[name] else None)
       return group_tensors[name][:3]
 
     outputs = {}

@@ -193,7 +193,7 @@ class EasyRecEstimator(object):
     self.model.eval()
     self.input_layer.drop_prefetch()   # (an id exchange prefetched for the next TRAINING batch is not this batch's)
     logits = self.model(feats)
-    self.input_layer._pending = []
+    self.input_layer.discard_pending()
     return logits
 
   def _group_fields(self):

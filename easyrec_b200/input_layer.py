@@ -81,6 +81,18 @@ def multi_feature(name, kind, embedding_dim, hash_bucket_size=0, num_buckets=0, 
 
 _COMBINER = {'sum': _lib.COMBINER_SUM, 'mean': _lib.COMBINER_MEAN, 'sqrtn': _lib.COMBINER_SQRTN}
 
+# The plan's records.  A column of a feature group's concat, `width` wide: kind 'emb' (looked up), 'dense' (raw values,
+# no table), 'seqc' (a SequenceFeature pooled by its sequence_combiner) or 'att' (target attention over the group's
+# sequence_features: `out_key` names their seq_layout, `need_key` appends the key).  A looked-up column reads `slot`
+# into columns [col, col + dim) of the (dim, out_key) output matrix.
+GroupColumn = collections.namedtuple('GroupColumn', ['name', 'kind', 'width', 'dim', 'out_key', 'col', 'need_key', 'slot'],
+                                     defaults=(None,) * 5)
+# a key or history column of a seq_layout, or a sequence column of a seq_group_layout
+SeqColumn = collections.namedtuple('SeqColumn', ['name', 'dim', 'out_key', 'col', 'slot'], defaults=(None, None))
+# one K7 update of a step: an arena's MergedCall - or, row-sharded with several launches on the arena, one launch's
+# _SubCall - with the rows, lookup weights, output matrices and segment ids of the lookup
+Pending = collections.namedtuple('Pending', ['call', 'rows', 'weights', 'outs', 'seg_ids'])
+
 
 class _SubCall(object):
   """One uniform launch over an arena: a list of slots that all have the same segment count."""
@@ -181,234 +193,26 @@ class InputLayer(object):
       self.raw_cols[n] = (c, c + self.features[n].raw_input_dim)
       c += self.features[n].raw_input_dim
     self.n_dense = c
-    B = batch_size
     # ---- table plan -------------------------------------------------------------------
     self.arenas = collections.OrderedDict()          # dim -> Arena
     self.subcalls = collections.OrderedDict()        # dim -> OrderedDict(key -> _SubCall)
-    self.group_layout = {}    # group -> list of (feature, kind, width, dim, out_key, col)
-    self.seq_layout = {}      # seq group -> dict(key=[(feature, dim, out_key, col)], hist=[...], T=..)
-    self.seq_group_layout = {}   # output_seq_and_normal_feature group -> dict(seq=[(feature, dim, out_key, col)], T=..)
-
-    def add_slot(dim, out_key, fname, table, kind, wide=False, pooled_seq=False):
-      f = self.features[fname]
-      arena = self.arenas.setdefault(dim, E.Arena(dim, device, shard_n, shard_rank))
-      arena.add_table(table, f.num_buckets)
-      if kind == 'seq' and fname in self.multi_valued_seq:
-        kind = 'mseq'
-        sk, nseg = ('mseq', f.seq_len), B * f.seq_len
-      elif kind == 'seq':
-        sk, nseg = ('seq', f.seq_len), B * f.seq_len
-      elif kind == 'tag':
-        sk, nseg = ('tag',), B
-      else:
-        sk, nseg = ('single',), B
-      subs = self.subcalls.setdefault(dim, collections.OrderedDict())
-      sc = subs.setdefault(sk, _SubCall(sk[0], nseg))
-      comb = _lib.COMBINER_SUM if (wide or f.kind == 'raw' or kind == 'seq') else _COMBINER[f.combiner]
-      slot = E.Slot(out_key + '/' + fname, table, f.bucket_mode, f.num_buckets, comb, out_buf=out_key,
-                    n_seg_per_sample=f.seq_len if kind in ('seq', 'mseq') else 1)
-      # id and sequence slots never carry per-lookup weights (raw-value and kv-weighted tag slots do)
-      slot.unit_weights = f.kind != 'raw' and kind in ('single', 'seq', 'mseq')
-      if f.kind == 'raw':
-        src = ('raw', self.raw_cols[fname][0])
-      elif kind in ('seq', 'mseq'):
-        src = ('seq', fname)
-      elif kind == 'tag':
-        src = ('tag', fname)
-      else:
-        src = ('id', self.sparse_names.index(fname))
-      sc.items.append((out_key, fname, slot, src))
-
+    self.group_layout = {}       # group -> [GroupColumn] in concat order
+    self.seq_layout = {}         # seq group -> dict(key=[SeqColumn], hist=[SeqColumn], T=steps)
+    self.seq_group_layout = {}   # output_seq_and_normal_feature group -> dict(seq=[SeqColumn], T=steps)
     self.attention_modules = collections.OrderedDict()
     self.seqc_order = {}      # group -> names of its sequence-combiner features in config order
+    self._shard = (shard_n, shard_rank)
     for gname, g in groups.items():
-      layout = []
-      seqc = []
-      wide = bool(g.get('wide'))
-      if gname in self.seq_output_groups:
-        if wide:
-          raise NotImplementedError('feature group %s: wide_deep WIDE read by output_seq_and_normal_feature' % gname)
-        if g.get('seq'):
-          raise NotImplementedError('feature group %s: sequence_features in a group read by '
-                                    'output_seq_and_normal_feature' % gname)
-        self.seq_group_layout[gname] = dict(seq=[], T=None)
-      for fname in g['features']:
-        f = self.features[fname]
-        dim = wide_output_dim if wide else f.embedding_dim
-        if f.kind == 'raw' and dim == 0:
-          layout.append((fname, 'dense', f.raw_input_dim, None, None, None))
-          continue
-        if f.kind == 'seq' and gname in self.seq_output_groups:
-          # InputLayer.get_sequence_feature (layers/input_layer.py:154-192): the un-pooled [B, T, D] lookup, in the
-          # table of the column itself (variable_scope('input_layer/' + column name): no group scope, so a feature
-          # listed in another group too reads the same table).  T is max_seq_len, fixed so the step can be captured.
-          sl = self.seq_group_layout[gname]
-          if fname in self.multi_valued_seq:
-            raise NotImplementedError('SequenceFeature %s: seq_multi_sep (multi-valued steps) in group %s read by '
-                                      'output_seq_and_normal_feature' % (fname, gname))
-          if sl['T'] not in (None, f.seq_len):
-            raise NotImplementedError('feature group %s: SequenceFeatures of different max_seq_len (%d, %d) read by '
-                                      'output_seq_and_normal_feature' % (gname, sl['T'], f.seq_len))
-          sl['T'] = f.seq_len
-          # all sequence features of one width write one [B*T, sum D] matrix: the concat costs nothing
-          add_slot(dim, gname + '#seq', fname, f.embedding_name or fname + '_embedding', 'seq')
-          sl['seq'].append([fname, dim, gname + '#seq', None])
-          continue
-        if f.kind == 'seq':
-          if self.seq_combiners.get(fname) != 'attention' or wide or fname in self.multi_valued_seq:
-            raise NotImplementedError('SequenceFeature %s in a plain group needs a sequence_combiner { attention } '
-                                      '(or put it in seq_att_groups / sequence_features)' % fname)
-          # un-pooled [B*T, D] rows in a matrix of their own; pooled in lookup() by the attention combiner.  In the
-          # concat these features follow the plain ones in NAME order, in the per-feature list in config order
-          # (input_layer.py:312, 364-367)
-          table = f.embedding_name or fname + '_embedding'
-          out_key = '%s#seqc/%s' % (gname, fname)
-          add_slot(dim, out_key, fname, table, 'seq')
-          seqc.append([fname, 'seqc', dim, dim, out_key, None])
-          from easyrec_b200 import layers as L
-          att = L.Dense(dim, 1, generator=dense_generator)
-          att.bias.requires_grad_(False)       # tf.layers.dense(units=1, use_bias=False, name='attention')
-          self.attention_modules[out_key] = att
-          continue
-        table = (f.embedding_name or fname + '_embedding') + ('_wide' if wide else '')
-        kind = 'tag' if f.kind == 'tag' else 'single'
-        # one output matrix per (group, launch kind): the single-valued and the CSR launch of a mixed group
-        # write their own matrices, the group's concat is assembled from both in config order
-        out_key = gname if kind == 'single' else gname + '#tag'
-        add_slot(dim, out_key, fname, table, kind, wide=wide)
-        layout.append([fname, 'emb', dim, dim, out_key, None])
-      self.seqc_order[gname] = [e[0] for e in seqc]
-      self.group_layout[gname] = layout + sorted(seqc, key=lambda e: e[0])
-      if gname in self.seq_group_layout and not self.seq_group_layout[gname]['seq']:
-        raise ValueError('[input_%s] sequence feature is empty (output_seq_and_normal_feature)' % gname)
+      self._plan_group(gname, g, dense_generator)
     for sname, maps in self.seq_att_groups.items():
-      lay = dict(key=[], hist=[], T=None)
-      for keys, hists in maps:
-        for k in keys:
-          f = self.features[k]
-          # the key column lives in the sequence group's own variable scope
-          # (layers/seq_input_layer.py:56-75): a table separate from the plain group's
-          table = f.embedding_name or '%s/%s_embedding' % (sname, k)
-          add_slot(f.embedding_dim, sname + '/key', k, table, 'single')
-          lay['key'].append([k, f.embedding_dim, sname + '/key', None])
-        for h in hists:
-          f = self.features[h]
-          assert f.kind == 'seq', '%s must be a SequenceFeature' % h
-          assert lay['T'] in (None, f.seq_len), 'hist_seq features of one group must share seq_len'
-          lay['T'] = f.seq_len
-          table = f.embedding_name or '%s/%s_embedding' % (sname, h)
-          add_slot(f.embedding_dim, sname + '/hist', h, table, 'seq')
-          lay['hist'].append([h, f.embedding_dim, sname + '/hist', None])
-      self.seq_layout[sname] = lay
-    # feature_groups[...].sequence_features: target attention INSIDE a group (layers/input_layer.py:96-111 ->
-    # SequenceFeatureLayer, layers/sequence_feature_layer.py:190-249 -> SeqInputLayer with scope_name = the group's):
-    # a key that is a feature of the same group reuses the group's own embedding output (seq_input_layer.py:63-75);
-    # histories live in the group's scope; the attended vector (+ the key) is appended to the group's concat
+      # the key column lives in the sequence group's own variable scope
+      # (layers/seq_input_layer.py:56-75): a table separate from the plain group's
+      self._plan_seq_layout(sname, sname, maps)
     for gname, g in groups.items():
       for sub in g.get('seq') or []:
-        if g.get('wide'):
-          raise NotImplementedError('sequence_features in the wide group %s' % gname)
-        from easyrec_b200 import layers as L
-        sname = '%s/%s' % (gname, sub['name'])
-        lay = dict(key=[], hist=[], T=None)
-        for keys, hists in sub['maps']:
-          for k in keys:
-            f = self.features[k]
-            own = [e for e in self.group_layout[gname] if e[0] == k and e[1] == 'emb']
-            if own:
-              if own[0][4] != gname:
-                raise NotImplementedError('sequence_features key %s is a multi-valued feature of group %s' % (k, gname))
-              lay['key'].append([k, own[0][3], gname, None])       # the column is filled in with the group's slot
-            else:
-              table = f.embedding_name or '%s/%s_embedding' % (gname, k)
-              add_slot(f.embedding_dim, sname + '/key', k, table, 'single')
-              lay['key'].append([k, f.embedding_dim, sname + '/key', None])
-          for h in hists:
-            f = self.features[h]
-            assert f.kind == 'seq', '%s must be a SequenceFeature' % h
-            assert lay['T'] in (None, f.seq_len), 'hist_seq features of one group must share seq_len'
-            lay['T'] = f.seq_len
-            table = f.embedding_name or '%s/%s_embedding' % (gname, h)
-            add_slot(f.embedding_dim, sname + '/hist', h, table, 'seq')
-            lay['hist'].append([h, f.embedding_dim, sname + '/hist', None])
-        dk, dh = sum(e[1] for e in lay['key']), sum(e[1] for e in lay['hist'])
-        if dk != dh:
-          raise NotImplementedError('sequence_features %s: key width %d != history width %d (allow_key_transform)'
-                                    % (sname, dk, dh))
-        self.seq_layout[sname] = lay
-        need_key = bool(sub.get('need_key', True))
-        self.group_layout[gname].append(['seq_fea/' + sub['name'], 'att', dh + (dk if need_key else 0), None, sname, need_key])
-        self.attention_modules[sname] = L.DNN(4 * dh, sub['units'], last_layer_no_activation=True,
-                                              last_layer_no_batch_norm=True, generator=dense_generator)
-    # ER_BUCKET_ONE_ROW promises that no other slot of the arena reads the table (a raw feature listed in two groups
-    # of the same width breaks that): such slots go through the ordinary dedup
-    for dim, subs in self.subcalls.items():
-      uses = collections.Counter(slot.table for sc in subs.values() for _, _, slot, _ in sc.items)
-      for sc in subs.values():
-        for _, _, slot, _ in sc.items:
-          if slot.bucket_mode == _lib.BUCKET_ONE_ROW and (uses[slot.table] > 1 or sc.kind != 'single'):
-            slot.bucket_mode = _lib.BUCKET_NONE
-    for a in self.arenas.values():
-      a.materialize(embedding_optimizer, generator=generator, adagrad_init=adagrad_init)
-      # tables of a backbone `embedding_layer` block: Keras Embedding's uniform(-limit, limit) initialiser
-      for tname, limit in (uniform_tables or {}).items():
-        if tname in a.tables and os.environ.get('ER_PLAN_ONLY') != '1':
-          off, local, _ = a.tables[tname]
-          rows = torch.empty(local, a.dim, dtype=torch.float32, device=device)
-          rows.uniform_(-limit, limit, generator=generator)
-          a.weight[off:off + local].copy_(rows)
-    # ---- launches ---------------------------------------------------------------------
-    self.calls = collections.OrderedDict()     # dim -> the single-valued ArenaCall (bench/tests)
-    self.merged = collections.OrderedDict()    # dim -> MergedCall
-    self._gather_plan = {}
-    self.static_ids = {}
-    self.static_w = {}
-    self.out_index = {}                        # (dim, out_key) -> (subcall key, local buf index)
-    for dim, subs in self.subcalls.items():
-      for sk, sc in subs.items():
-        keys = []
-        for out_key, _, _, _ in sc.items:
-          if out_key not in keys:
-            keys.append(out_key)
-        widths = [0] * len(keys)
-        slots = []
-        for out_key, fname, slot, src in sc.items:
-          slot.out_buf = keys.index(out_key)
-          widths[slot.out_buf] += dim
-          slots.append(slot)
-        if sc.kind == 'tag':
-          cap = max_tag_lookups or 8 * B * len(slots)
-          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=False, max_lookups=cap)
-        elif sc.kind == 'mseq':
-          cap = max_tag_lookups or 4 * B * sk[1] * len(slots)     # room for 4 values per step on average
-          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=False, max_lookups=cap)
-        else:
-          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=True)
-        for i, (out_key, fname, slot, src) in enumerate(sc.items):
-          col = sc.call.slot_cols[i]
-          for lay in list(self.group_layout.values()):
-            for e in lay:
-              if e[1] in ('emb', 'seqc') and e[0] == fname and e[4] == out_key and e[5] is None:
-                e[5] = col
-          for lay in list(self.seq_layout.values()) + list(self.seq_group_layout.values()):
-            for part in ('key', 'hist', 'seq'):
-              for e in lay.get(part, ()):
-                if e[0] == fname and e[2] == out_key and e[3] is None:
-                  e[3] = col
-        for j, k in enumerate(keys):
-          self.out_index[(dim, k)] = (sk, j)
-        if sc.kind == 'single':
-          self.calls[dim] = sc.call
-          src = [s for _, _, _, s in sc.items]
-          self.static_ids[dim] = torch.zeros(sc.call.n_seg, dtype=torch.int64, device=device)
-          has_raw = any(k == 'raw' for k, _ in src)
-          self.static_w[dim] = (torch.ones(sc.call.n_seg, dtype=torch.float32, device=device)
-                                if has_raw else None)
-          sc.call.identity_ids = ([k for k, _ in src] == ['id'] * len(src) and
-                                  [i for _, i in src] == list(range(len(self.sparse_names))))
-          sc.call.sources = src
-      self.merged[dim] = MergedCall(self.arenas[dim], list(subs.values()))
-    self.call_feature_idx = {d: c.sources for d, c in self.calls.items()}
+        self._plan_sequence_features(gname, g, sub, dense_generator)
+    self._materialize(embedding_optimizer, generator, adagrad_init, uniform_tables)
+    self._plan_calls(max_tag_lookups)
     mn = [self.features[n].min_val for n in self.raw_names for _ in range(self.features[n].raw_input_dim)]
     mx = [self.features[n].max_val for n in self.raw_names for _ in range(self.features[n].raw_input_dim)]
     rng = np.array(mx, np.float32) - np.array(mn, np.float32)
@@ -425,45 +229,13 @@ class InputLayer(object):
     # and every lookup goes through the all-to-all exchange of sharded.ShardedLookup
     self.ep = shard_n > 1
     if self.ep:
-      from easyrec_b200.sharded import ShardedLookup
-      exchanges = {}   # row plan -> the exchange its arenas share (ids once, rows in one packed all-to-all)
-      for dim, subs in self.subcalls.items():
-        for sk, sc in subs.items():
-          if sc.kind != 'single':
-            # multi-valued slots (the ragged forms of embedding_parallel_lookup) and un-pooled histories (one lookup per
-            # step, padded steps dropped by K1): an exchange of their own.  The owner applies one row update per
-            # exchange, so a table must not be read by slots of two different launches
-            mine = set(slot.table for _, _, slot, _ in sc.items)
-            for sk2, sc2 in subs.items():
-              shared = sorted(mine & set(slot.table for _, _, slot, _ in sc2.items)) if sc2 is not sc else None
-              if shared and 'seq' in (sc.kind, sc2.kind):
-                raise NotImplementedError('EmbeddingParallel: table(s) %s are read both by history (SequenceFeature) '
-                                          'steps and by other features; give the histories tables of their own'
-                                          % shared)
-              if shared:
-                raise NotImplementedError('EmbeddingParallel: table(s) %s are shared by single- and multi-valued features'
-                                          % shared)
-            if sc.kind == 'seq' and len(subs) > 1 and self.arenas[dim].opt_kind == _lib.OPT_ADAM_ROWS:
-              # adam_optimizer's dense decay sweeps every row the owner did not update: with two exchanges on one arena
-              # each would sweep the rows only the other one updated
-              raise NotImplementedError('EmbeddingParallel: adam_optimizer with histories next to other features of '
-                                        'embedding_dim %d (their tables share one arena and two exchanges)' % dim)
-            seq = (B, sk[1]) if sc.kind == 'seq' else None
-            sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, seq=seq)
-            if len(subs) == 1:
-              self.merged[dim].sharded = sc.sharded
-            continue
-          key = self._rows_key(sc)
-          sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, exchange=exchanges.get(key))
-          exchanges.setdefault(key, sc.sharded.ex)
-          self.merged[dim].sharded = sc.sharded
-      self._ep_scale = 1.0 / shard_n
+      self._plan_exchanges()
     # embedding_learning_rate_multiplier: the reference multiplies the GRADIENT of every `embedding_weights`
     # variable by it (model/easy_rec_estimator.py:308-317 gradient_multipliers), before the optimizer rule
     self.emb_grad_mult = 1.0
     # 1/N of data-parallel replicas or of row-sharded tables (compat/optimizers.py:289-292,315-316)
-    self.replica_grad_scale = getattr(self, '_ep_scale', 1.0)
-    self._pending = []
+    self.replica_grad_scale = 1.0 / shard_n
+    self._pending = []        # [Pending] of the last lookup(): what backward_update() applies
     self._rows_cache = {}
     self.placements = E.Placements()
     self._side = None
@@ -473,6 +245,260 @@ class InputLayer(object):
     self._pos = {}
     self._next_ids = {}
     self._clip_state = {}
+
+  # ---- table plan: the constructor's stages ---------------------------------------------
+  def _add_slot(self, dim, out_key, fname, table, kind, wide=False):
+    """one lookup of feature `fname` from `table` into the (dim, out_key) output matrix; returns its Slot"""
+    f = self.features[fname]
+    B = self.batch_size
+    arena = self.arenas.setdefault(dim, E.Arena(dim, self.device, *self._shard))
+    arena.add_table(table, f.num_buckets)
+    if kind == 'seq' and fname in self.multi_valued_seq:
+      kind = 'mseq'
+      sk, nseg = ('mseq', f.seq_len), B * f.seq_len
+    elif kind == 'seq':
+      sk, nseg = ('seq', f.seq_len), B * f.seq_len
+    elif kind == 'tag':
+      sk, nseg = ('tag',), B
+    else:
+      sk, nseg = ('single',), B
+    subs = self.subcalls.setdefault(dim, collections.OrderedDict())
+    sc = subs.setdefault(sk, _SubCall(sk[0], nseg))
+    comb = _lib.COMBINER_SUM if (wide or f.kind == 'raw' or kind == 'seq') else _COMBINER[f.combiner]
+    slot = E.Slot(out_key + '/' + fname, table, f.bucket_mode, f.num_buckets, comb, out_buf=out_key,
+                  n_seg_per_sample=f.seq_len if kind in ('seq', 'mseq') else 1)
+    # id and sequence slots never carry per-lookup weights (raw-value and kv-weighted tag slots do)
+    slot.unit_weights = f.kind != 'raw' and kind in ('single', 'seq', 'mseq')
+    if f.kind == 'raw':
+      src = ('raw', self.raw_cols[fname][0])
+    elif kind in ('seq', 'mseq'):
+      src = ('seq', fname)
+    elif kind == 'tag':
+      src = ('tag', fname)
+    else:
+      src = ('id', self.sparse_names.index(fname))
+    sc.items.append((out_key, fname, slot, src))
+    return slot
+
+  def _plan_group(self, gname, g, dense_generator):
+    """the columns of one feature group, in config order"""
+    layout, seqc, seq, T = [], [], [], None
+    wide = bool(g.get('wide'))
+    if gname in self.seq_output_groups:
+      if wide:
+        raise NotImplementedError('feature group %s: wide_deep WIDE read by output_seq_and_normal_feature' % gname)
+      if g.get('seq'):
+        raise NotImplementedError('feature group %s: sequence_features in a group read by '
+                                  'output_seq_and_normal_feature' % gname)
+    for fname in g['features']:
+      f = self.features[fname]
+      dim = self.wide_output_dim if wide else f.embedding_dim
+      if f.kind == 'raw' and dim == 0:
+        layout.append(GroupColumn(fname, 'dense', f.raw_input_dim))
+        continue
+      if f.kind == 'seq' and gname in self.seq_output_groups:
+        # InputLayer.get_sequence_feature (layers/input_layer.py:154-192): the un-pooled [B, T, D] lookup, in the
+        # table of the column itself (variable_scope('input_layer/' + column name): no group scope, so a feature
+        # listed in another group too reads the same table).  T is max_seq_len, fixed so the step can be captured.
+        if fname in self.multi_valued_seq:
+          raise NotImplementedError('SequenceFeature %s: seq_multi_sep (multi-valued steps) in group %s read by '
+                                    'output_seq_and_normal_feature' % (fname, gname))
+        if T not in (None, f.seq_len):
+          raise NotImplementedError('feature group %s: SequenceFeatures of different max_seq_len (%d, %d) read by '
+                                    'output_seq_and_normal_feature' % (gname, T, f.seq_len))
+        T = f.seq_len
+        # all sequence features of one width write one [B*T, sum D] matrix: the concat costs nothing
+        slot = self._add_slot(dim, gname + '#seq', fname, f.embedding_name or fname + '_embedding', 'seq')
+        seq.append(SeqColumn(fname, dim, gname + '#seq', slot=slot))
+        continue
+      if f.kind == 'seq':
+        if self.seq_combiners.get(fname) != 'attention' or wide or fname in self.multi_valued_seq:
+          raise NotImplementedError('SequenceFeature %s in a plain group needs a sequence_combiner { attention } '
+                                    '(or put it in seq_att_groups / sequence_features)' % fname)
+        # un-pooled [B*T, D] rows in a matrix of their own; pooled in lookup() by the attention combiner.  In the
+        # concat these features follow the plain ones in NAME order, in the per-feature list in config order
+        # (input_layer.py:312, 364-367)
+        out_key = '%s#seqc/%s' % (gname, fname)
+        slot = self._add_slot(dim, out_key, fname, f.embedding_name or fname + '_embedding', 'seq')
+        seqc.append(GroupColumn(fname, 'seqc', dim, dim, out_key, slot=slot))
+        from easyrec_b200 import layers as L
+        att = L.Dense(dim, 1, generator=dense_generator)
+        att.bias.requires_grad_(False)       # tf.layers.dense(units=1, use_bias=False, name='attention')
+        self.attention_modules[out_key] = att
+        continue
+      table = (f.embedding_name or fname + '_embedding') + ('_wide' if wide else '')
+      kind = 'tag' if f.kind == 'tag' else 'single'
+      # one output matrix per (group, launch kind): the single-valued and the CSR launch of a mixed group
+      # write their own matrices, the group's concat is assembled from both in config order
+      out_key = gname if kind == 'single' else gname + '#tag'
+      slot = self._add_slot(dim, out_key, fname, table, kind, wide=wide)
+      layout.append(GroupColumn(fname, 'emb', dim, dim, out_key, slot=slot))
+    self.seqc_order[gname] = [e.name for e in seqc]
+    self.group_layout[gname] = layout + sorted(seqc, key=lambda e: e.name)
+    if gname in self.seq_output_groups:
+      if not seq:
+        raise ValueError('[input_%s] sequence feature is empty (output_seq_and_normal_feature)' % gname)
+      self.seq_group_layout[gname] = dict(seq=seq, T=T)
+
+  def _plan_seq_layout(self, sname, scope, maps, own=()):
+    """SeqInputLayer (layers/seq_input_layer.py:34-124) over `maps` [(key names, hist_seq names)]: key and history
+    columns in tables of the variable scope `scope`; a key that is one of the `own` group columns reuses it"""
+    key, hist, T = [], [], None
+    for keys, hists in maps:
+      for k in keys:
+        f = self.features[k]
+        mine = next((e for e in own if e.name == k and e.kind == 'emb'), None)
+        if mine is not None:
+          if mine.out_key != scope:
+            raise NotImplementedError('sequence_features key %s is a multi-valued feature of group %s' % (k, scope))
+          key.append(SeqColumn(k, mine.dim, mine.out_key, slot=mine.slot))
+          continue
+        table = f.embedding_name or '%s/%s_embedding' % (scope, k)
+        slot = self._add_slot(f.embedding_dim, sname + '/key', k, table, 'single')
+        key.append(SeqColumn(k, f.embedding_dim, sname + '/key', slot=slot))
+      for h in hists:
+        f = self.features[h]
+        assert f.kind == 'seq', '%s must be a SequenceFeature' % h
+        assert T in (None, f.seq_len), 'hist_seq features of one group must share seq_len'
+        T = f.seq_len
+        table = f.embedding_name or '%s/%s_embedding' % (scope, h)
+        slot = self._add_slot(f.embedding_dim, sname + '/hist', h, table, 'seq')
+        hist.append(SeqColumn(h, f.embedding_dim, sname + '/hist', slot=slot))
+    self.seq_layout[sname] = lay = dict(key=key, hist=hist, T=T)
+    return lay
+
+  def _plan_sequence_features(self, gname, g, sub, dense_generator):
+    """feature_groups[...].sequence_features: target attention INSIDE a group (layers/input_layer.py:96-111 ->
+    SequenceFeatureLayer, layers/sequence_feature_layer.py:190-249 -> SeqInputLayer with scope_name = the group's):
+    a key that is a feature of the same group reuses the group's own embedding output (seq_input_layer.py:63-75);
+    histories live in the group's scope; the attended vector (+ the key) is appended to the group's concat"""
+    if g.get('wide'):
+      raise NotImplementedError('sequence_features in the wide group %s' % gname)
+    from easyrec_b200 import layers as L
+    sname = '%s/%s' % (gname, sub['name'])
+    lay = self._plan_seq_layout(sname, gname, sub['maps'], own=self.group_layout[gname])
+    dk, dh = sum(e.dim for e in lay['key']), sum(e.dim for e in lay['hist'])
+    if dk != dh:
+      raise NotImplementedError('sequence_features %s: key width %d != history width %d (allow_key_transform)'
+                                % (sname, dk, dh))
+    need_key = bool(sub.get('need_key', True))
+    self.group_layout[gname].append(GroupColumn('seq_fea/' + sub['name'], 'att', dh + (dk if need_key else 0),
+                                                out_key=sname, need_key=need_key))
+    self.attention_modules[sname] = L.DNN(4 * dh, sub['units'], last_layer_no_activation=True,
+                                          last_layer_no_batch_norm=True, generator=dense_generator)
+
+  def _materialize(self, embedding_optimizer, generator, adagrad_init, uniform_tables):
+    # ER_BUCKET_ONE_ROW promises that no other slot of the arena reads the table (a raw feature listed in two groups
+    # of the same width breaks that): such slots go through the ordinary dedup
+    for subs in self.subcalls.values():
+      uses = collections.Counter(slot.table for sc in subs.values() for _, _, slot, _ in sc.items)
+      for sc in subs.values():
+        for _, _, slot, _ in sc.items:
+          if slot.bucket_mode == _lib.BUCKET_ONE_ROW and (uses[slot.table] > 1 or sc.kind != 'single'):
+            slot.bucket_mode = _lib.BUCKET_NONE
+    for a in self.arenas.values():
+      a.materialize(embedding_optimizer, generator=generator, adagrad_init=adagrad_init)
+      # tables of a backbone `embedding_layer` block: Keras Embedding's uniform(-limit, limit) initialiser
+      for tname, limit in (uniform_tables or {}).items():
+        if tname in a.tables and os.environ.get('ER_PLAN_ONLY') != '1':
+          off, local, _ = a.tables[tname]
+          rows = torch.empty(local, a.dim, dtype=torch.float32, device=self.device)
+          rows.uniform_(-limit, limit, generator=generator)
+          a.weight[off:off + local].copy_(rows)
+
+  def _plan_calls(self, max_tag_lookups):
+    """one ArenaCall per sub-call (its output matrices in first-use order), one MergedCall per arena"""
+    B, device = self.batch_size, self.device
+    self.calls = collections.OrderedDict()     # dim -> the single-valued ArenaCall (bench/tests)
+    self.merged = collections.OrderedDict()    # dim -> MergedCall
+    self._gather_plan = {}
+    self.static_ids = {}
+    self.static_w = {}
+    self.out_index = {}                        # (dim, out_key) -> (subcall key, local buf index)
+    for dim, subs in self.subcalls.items():
+      for sk, sc in subs.items():
+        keys = list(dict.fromkeys(out_key for out_key, _, _, _ in sc.items))
+        widths = [0] * len(keys)
+        slots = []
+        for out_key, _, slot, _ in sc.items:
+          slot.out_buf = keys.index(out_key)
+          widths[slot.out_buf] += dim
+          slots.append(slot)
+        if sc.kind == 'tag':
+          cap = max_tag_lookups or 8 * B * len(slots)
+          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=False, max_lookups=cap)
+        elif sc.kind == 'mseq':
+          cap = max_tag_lookups or 4 * B * sk[1] * len(slots)     # room for 4 values per step on average
+          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=False, max_lookups=cap)
+        else:
+          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=True)
+        for j, k in enumerate(keys):
+          self.out_index[(dim, k)] = (sk, j)
+        if sc.kind == 'single':
+          self.calls[dim] = sc.call
+          src = [s for _, _, _, s in sc.items]
+          self.static_ids[dim] = torch.zeros(sc.call.n_seg, dtype=torch.int64, device=device)
+          has_raw = any(k == 'raw' for k, _ in src)
+          self.static_w[dim] = (torch.ones(sc.call.n_seg, dtype=torch.float32, device=device)
+                                if has_raw else None)
+          sc.call.identity_ids = ([k for k, _ in src] == ['id'] * len(src) and
+                                  [i for _, i in src] == list(range(len(self.sparse_names))))
+          sc.call.sources = src
+      self.merged[dim] = MergedCall(self.arenas[dim], list(subs.values()))
+    # every looked-up column reads its position from its own slot's ArenaCall
+    cols = {id(slot): c for subs in self.subcalls.values() for sc in subs.values()
+            for slot, c in zip(sc.call.slots, sc.call.slot_cols)}
+
+    def resolved(columns):
+      return [e if e.slot is None else e._replace(col=cols[id(e.slot)]) for e in columns]
+    self.group_layout = {g: resolved(lay) for g, lay in self.group_layout.items()}
+    self.seq_layout = {s: dict(lay, key=resolved(lay['key']), hist=resolved(lay['hist']))
+                       for s, lay in self.seq_layout.items()}
+    self.seq_group_layout = {g: dict(lay, seq=resolved(lay['seq'])) for g, lay in self.seq_group_layout.items()}
+
+  def _plan_exchanges(self):
+    """EmbeddingParallel: a ShardedLookup around every sub-call"""
+    from easyrec_b200.sharded import ShardedLookup
+    shard_n, shard_rank = self._shard
+    exchanges = {}   # row plan -> the exchange its arenas share (ids once, rows in one packed all-to-all)
+    for dim, subs in self.subcalls.items():
+      for sk, sc in subs.items():
+        if sc.kind != 'single':
+          # multi-valued slots (the ragged forms of embedding_parallel_lookup) and un-pooled histories (one lookup per
+          # step, padded steps dropped by K1): an exchange of their own.  The owner applies one row update per
+          # exchange, so a table must not be read by slots of two different launches
+          mine = set(slot.table for _, _, slot, _ in sc.items)
+          for sk2, sc2 in subs.items():
+            shared = sorted(mine & set(slot.table for _, _, slot, _ in sc2.items)) if sc2 is not sc else None
+            if shared and 'seq' in (sc.kind, sc2.kind):
+              raise NotImplementedError('EmbeddingParallel: table(s) %s are read both by history (SequenceFeature) '
+                                        'steps and by other features; give the histories tables of their own'
+                                        % shared)
+            if shared:
+              raise NotImplementedError('EmbeddingParallel: table(s) %s are shared by single- and multi-valued features'
+                                        % shared)
+          if sc.kind == 'seq' and len(subs) > 1 and self.arenas[dim].opt_kind == _lib.OPT_ADAM_ROWS:
+            # adam_optimizer's dense decay sweeps every row the owner did not update: with two exchanges on one arena
+            # each would sweep the rows only the other one updated
+            raise NotImplementedError('EmbeddingParallel: adam_optimizer with histories next to other features of '
+                                      'embedding_dim %d (their tables share one arena and two exchanges)' % dim)
+          seq = (self.batch_size, sk[1]) if sc.kind == 'seq' else None
+          sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, seq=seq)
+          if len(subs) == 1:
+            self.merged[dim].sharded = sc.sharded
+          continue
+        key = self._rows_key(sc)
+        sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, exchange=exchanges.get(key))
+        exchanges.setdefault(key, sc.sharded.ex)
+        self.merged[dim].sharded = sc.sharded
+
+  def group_width(self, name):
+    """width of the group's concat [B, width]"""
+    return sum(e.width for e in self.group_layout[name])
+
+  def discard_pending(self):
+    """forget the K7 updates of the last lookup() without applying them (evaluation, or updates applied elsewhere)"""
+    self._pending = []
 
   # ------------------------------------------------------------------
   def set_optimizer_step(self, lr, step, beta1=0.9, beta2=0.999, eps=1e-8, grad_scale=1.0):
@@ -796,6 +822,24 @@ class InputLayer(object):
       outs = E.fused_lookup(call, rows)
       return rows, None, None, None, outs
     # tag: CSR
+    cap = call.max_lookups
+    ids_cap, lens, weights = self._csr_inputs(sc, features)
+    row_ptr, seg_ids = K.csr_from_lens(lens.contiguous(), cap)
+    if self.ep:
+      # row-sharded tables: K1 (owner, local row) -> K8 -> all-to-alls -> pooling of the received rows by the same CSR
+      outs = call.alloc_outputs()
+      rows = sc.sharded.forward(ids_cap, weights, outs, row_ptr=row_ptr, seg_ids=seg_ids)
+      for o in outs:
+        o.requires_grad_(True)
+      return rows, weights, row_ptr, seg_ids, outs
+    rows = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
+    K.bucketize(ids_cap, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr,
+                rows=rows, **K.k1_weight_args(ids_cap, weights))
+    outs = E.fused_lookup(call, rows, weights=weights, row_ptr=row_ptr)
+    return rows, weights, row_ptr, seg_ids, outs
+
+  def _csr_inputs(self, sc, features):
+    """a multi-valued launch's ids padded to its lookup capacity, its lengths, and its weights (None: all 1)"""
     ids_list, lens_list, w_list = [], [], []
     any_w = False
     for _, fname, _, _ in sc.items:
@@ -812,7 +856,7 @@ class InputLayer(object):
     ids = torch.cat(ids_list) if len(ids_list) > 1 else ids_list[0]
     lens = torch.cat(lens_list) if len(lens_list) > 1 else lens_list[0]
     L = ids.numel()
-    cap = call.max_lookups
+    cap = sc.call.max_lookups
     assert L <= cap, 'tag lookups %d exceed max_tag_lookups %d' % (L, cap)
     weights = None
     if any_w:
@@ -824,19 +868,7 @@ class InputLayer(object):
         off += i_.numel()
     ids_cap = torch.zeros(cap, dtype=torch.int64, device=self.device)
     ids_cap[:L].copy_(ids)
-    row_ptr, seg_ids = K.csr_from_lens(lens.contiguous(), cap)
-    if self.ep:
-      # row-sharded tables: K1 (owner, local row) -> K8 -> all-to-alls -> pooling of the received rows by the same CSR
-      outs = call.alloc_outputs()
-      rows = sc.sharded.forward(ids_cap, weights, outs, row_ptr=row_ptr, seg_ids=seg_ids)
-      for o in outs:
-        o.requires_grad_(True)
-      return rows, weights, row_ptr, seg_ids, outs
-    rows = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
-    K.bucketize(ids_cap, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr,
-                rows=rows, **K.k1_weight_args(ids_cap, weights))
-    outs = E.fused_lookup(call, rows, weights=weights, row_ptr=row_ptr)
-    return rows, weights, row_ptr, seg_ids, outs
+    return ids_cap, lens, weights
 
   def has_group(self, group_name):
     return group_name in self.group_layout or group_name in self.seq_layout
@@ -865,7 +897,7 @@ class InputLayer(object):
     if not is_combine:
       return [], concat, per_feature
     if is_dict:
-      names = [e[0] for e in self.group_layout[group_name]]
+      names = [e.name for e in self.group_layout[group_name]]
       return concat, per_feature, dict(zip(names, per_feature))
     return concat, per_feature
 
@@ -879,7 +911,6 @@ class InputLayer(object):
     self._pending = []
     outs_by_key = {}
     for dim, subs in self.subcalls.items():
-      m = self.merged[dim]
       parts = []
       for sk, sc in subs.items():
         rows, w, row_ptr, seg_ids, outs = self._run_subcall(dim, sk, sc, features, dense_norm)
@@ -887,110 +918,118 @@ class InputLayer(object):
         for (d, k), (skk, j) in self.out_index.items():
           if d == dim and skk == sk:
             outs_by_key[(dim, k)] = outs[j]
-      if self.ep and len(parts) > 1:
-        # row-sharded tables: every launch has its own exchange and its own owner-side update (disjoint tables)
-        for sc, rows, w, seg_ids, outs in parts:
-          self._pending.append((sc, rows, w, outs, seg_ids))
-      elif len(parts) == 1:
-        sc, rows, w, seg_ids, outs = parts[0]
-        self._pending.append((m, rows, w, outs, seg_ids))
-      else:
-        all_outs = []
-        any_w = any(p[2] is not None for p in parts)
-        if any_w and m.weights is None:
-          m.weights = torch.ones(m.max_lookups, dtype=torch.float32, device=self.device)
-        for si, (sc, rows, w, seg_ids, outs) in enumerate(parts):
-          lo = m.sub_lookup_off[si]
-          n = rows.numel()
-          m.rows[lo:lo + n].copy_(rows)
-          if any_w:
-            if w is not None:
-              m.weights[lo:lo + n].copy_(w)
-            else:
-              m.weights[lo:lo + n].fill_(1.0)
-          if m.has_csr:
-            if seg_ids is not None:
-              m.seg_ids[lo:lo + n].copy_(seg_ids[:n] + m.sub_seg_off[si])
-            else:
-              m.seg_ids[lo:lo + n].copy_(
-                  torch.arange(m.sub_seg_off[si], m.sub_seg_off[si] + n, device=self.device,
-                               dtype=torch.int32))
-          if m.needs_scale:
-            so = m.sub_seg_off[si]
-            if sc.call.seg_scale is not None:
-              m.seg_scale[so:so + sc.call.n_seg].copy_(sc.call.seg_scale)
-          all_outs.extend(outs)
-        self._pending.append((m, m.rows, m.weights if any_w else None, all_outs,
-                              m.seg_ids if m.has_csr else None))
+      self._queue_update(self.merged[dim], parts)
     self._presort()
     self.seq_outputs = {}
     B = self.batch_size
     for sname, lay in self.seq_layout.items():
-      keys = [outs_by_key[(d, ok)][:, c:c + d] for (_, d, ok, c) in lay['key']]
-      hists = [outs_by_key[(d, ok)][:, c:c + d].reshape(B, lay['T'], d) for (_, d, ok, c) in lay['hist']]
-      lens = features['seq_fea'][lay['hist'][0][0]][1]
+      keys = [outs_by_key[(e.dim, e.out_key)][:, e.col:e.col + e.dim] for e in lay['key']]
+      hists = [outs_by_key[(e.dim, e.out_key)][:, e.col:e.col + e.dim].reshape(B, lay['T'], e.dim) for e in lay['hist']]
+      lens = features['seq_fea'][lay['hist'][0].name][1]
       self.seq_outputs[sname] = dict(
           key=keys[0] if len(keys) == 1 else torch.cat(keys, dim=-1),
           hist_seq_emb=hists[0] if len(hists) == 1 else torch.cat(hists, dim=-1),
           hist_seq_len=lens)
-    out = {}
-    for gname, layout in self.group_layout.items():
-      per_feature, mats, kinds, reg = [], {}, [], None
-      for (fname, kind, width, dim, out_key, col) in layout:
-        if kind == 'dense':
-          c0, c1 = self.raw_cols[fname]
-          v = dense_norm[:, c0:c1]
-        elif kind == 'seqc':
-          # sequence_combiner { attention } (input_layer.py:323-339): logits = dense(seq, 1, no bias), positions beyond
-          # the length masked with -2^32 + 1, softmax over the steps, weighted sum of the step embeddings
-          from easyrec_b200 import interactions as I
-          mat = outs_by_key[(dim, out_key)]
-          T = self.features[fname].seq_len
-          seq = mat[:, col:col + width].reshape(B, T, width).contiguous()
-          scores = self.attention_modules[out_key](seq.reshape(B * T, width)).reshape(B, T)
-          v = I.din_pool(scores.contiguous(), seq, features['seq_fea'][fname][1])
-          reg = (reg or []) + [seq]           # embedding_reg_lst takes the un-pooled sequence (input_layer.py:316)
-        elif kind == 'att':
-          # target attention over the group's sequence_features (sequence_feature_layer.py:123-189): softmax of the
-          # masked attention-MLP scores over the history, [attended history | key] (need_key_feature)
-          from easyrec_b200 import interactions as I
-          so = self.seq_outputs[out_key]
-          key = so['key'].contiguous()
-          att = I.din_attention(key, so['hist_seq_emb'].contiguous(), so['hist_seq_len'], self.attention_modules[out_key])
-          v = torch.cat([att, key], dim=1) if col else att
-          reg = (reg or []) + [so['hist_seq_emb']]
-        else:
-          mat = outs_by_key[(dim, out_key)]
-          mats[(dim, out_key)] = mat
-          v = mat[:, col:col + width]
-        per_feature.append(v)
-        kinds.append(kind)
-      if not layout:   # (only sequence features, read by output_seq_and_normal_feature)
-        concat = None
-      elif len(mats) == 1 and all(k == 'emb' for k in kinds):
-        (dim, out_key), mat = next(iter(mats.items()))
-        width = sum(e[2] for e in layout)
-        concat = mat if mat.shape[1] == width else mat[:, :width]
+    return {gname: self._group_outputs(gname, features, outs_by_key, dense_norm) for gname in self.group_layout}
+
+  def _queue_update(self, m, parts):
+    """the Pending K7 update(s) of one arena's launches `parts` [(sub-call, rows, weights, seg_ids, outs)]: several
+    launches are packed into the arena's MergedCall"""
+    if self.ep and len(parts) > 1:
+      # row-sharded tables: every launch has its own exchange and its own owner-side update (disjoint tables)
+      for sc, rows, w, seg_ids, outs in parts:
+        self._pending.append(Pending(sc, rows, w, outs, seg_ids))
+    elif len(parts) == 1:
+      sc, rows, w, seg_ids, outs = parts[0]
+      self._pending.append(Pending(m, rows, w, outs, seg_ids))
+    else:
+      all_outs = []
+      any_w = any(p[2] is not None for p in parts)
+      if any_w and m.weights is None:
+        m.weights = torch.ones(m.max_lookups, dtype=torch.float32, device=self.device)
+      for si, (sc, rows, w, seg_ids, outs) in enumerate(parts):
+        lo = m.sub_lookup_off[si]
+        n = rows.numel()
+        m.rows[lo:lo + n].copy_(rows)
+        if any_w:
+          if w is not None:
+            m.weights[lo:lo + n].copy_(w)
+          else:
+            m.weights[lo:lo + n].fill_(1.0)
+        if m.has_csr:
+          if seg_ids is not None:
+            m.seg_ids[lo:lo + n].copy_(seg_ids[:n] + m.sub_seg_off[si])
+          else:
+            m.seg_ids[lo:lo + n].copy_(
+                torch.arange(m.sub_seg_off[si], m.sub_seg_off[si] + n, device=self.device,
+                             dtype=torch.int32))
+        if m.needs_scale:
+          so = m.sub_seg_off[si]
+          if sc.call.seg_scale is not None:
+            m.seg_scale[so:so + sc.call.n_seg].copy_(sc.call.seg_scale)
+        all_outs.extend(outs)
+      self._pending.append(Pending(m, m.rows, m.weights if any_w else None, all_outs,
+                                   m.seg_ids if m.has_csr else None))
+
+  def _group_outputs(self, gname, features, outs_by_key, dense_norm):
+    """lookup()'s value for one feature group: (concat, [per-feature]), or (seq, seq_len, concat, [per-feature]) for a
+    group read by output_seq_and_normal_feature"""
+    B = self.batch_size
+    layout = self.group_layout[gname]
+    per_feature, mats, kinds, reg = [], {}, [], None
+    for e in layout:
+      if e.kind == 'dense':
+        c0, c1 = self.raw_cols[e.name]
+        v = dense_norm[:, c0:c1]
+      elif e.kind == 'seqc':
+        # sequence_combiner { attention } (input_layer.py:323-339): logits = dense(seq, 1, no bias), positions beyond
+        # the length masked with -2^32 + 1, softmax over the steps, weighted sum of the step embeddings
+        from easyrec_b200 import interactions as I
+        mat = outs_by_key[(e.dim, e.out_key)]
+        T = self.features[e.name].seq_len
+        seq = mat[:, e.col:e.col + e.width].reshape(B, T, e.width).contiguous()
+        scores = self.attention_modules[e.out_key](seq.reshape(B * T, e.width)).reshape(B, T)
+        v = I.din_pool(scores.contiguous(), seq, features['seq_fea'][e.name][1])
+        reg = (reg or []) + [seq]           # embedding_reg_lst takes the un-pooled sequence (input_layer.py:316)
+      elif e.kind == 'att':
+        # target attention over the group's sequence_features (sequence_feature_layer.py:123-189): softmax of the
+        # masked attention-MLP scores over the history, [attended history | key] (need_key_feature)
+        from easyrec_b200 import interactions as I
+        so = self.seq_outputs[e.out_key]
+        key = so['key'].contiguous()
+        att = I.din_attention(key, so['hist_seq_emb'].contiguous(), so['hist_seq_len'], self.attention_modules[e.out_key])
+        v = torch.cat([att, key], dim=1) if e.need_key else att
+        reg = (reg or []) + [so['hist_seq_emb']]
       else:
-        concat = torch.cat(per_feature, dim=1)
-      if reg is not None:
-        # the embedding regulariser covers what was LOOKED UP (the group's columns and the histories,
-        # input_layer.py:369-375, sequence_feature_layer.py:215-217), not the attended vectors appended to the concat
-        concat._er_reg = [v for v, k in zip(per_feature, kinds) if k == 'emb'] + reg
-      order = self.seqc_order.get(gname)
-      if order and len(order) > 1:
-        # the per-feature list keeps the sequence-combiner features in config order (the concat has them by name)
-        by_name = {e[0]: v for e, v in zip(layout, per_feature) if e[1] == 'seqc'}
-        per_feature = [v for e, v in zip(layout, per_feature) if e[1] != 'seqc'] + [by_name[n] for n in order]
-      if gname in self.seq_group_layout:
-        seq, seq_len = self._seq_group_tensors(gname, features, outs_by_key)
-        # the embedding regulariser covers the un-pooled sequence embeddings and the plain embedding columns
-        # (input_layer.py:117-151, 176-191)
-        seq._er_reg = [seq] + [v for v, k in zip(per_feature, kinds) if k == 'emb']
-        out[gname] = (seq, seq_len, concat, per_feature)
-        continue
-      out[gname] = (concat, per_feature)
-    return out
+        mat = outs_by_key[(e.dim, e.out_key)]
+        mats[(e.dim, e.out_key)] = mat
+        v = mat[:, e.col:e.col + e.width]
+      per_feature.append(v)
+      kinds.append(e.kind)
+    if not layout:   # (only sequence features, read by output_seq_and_normal_feature)
+      concat = None
+    elif len(mats) == 1 and all(k == 'emb' for k in kinds):
+      mat = next(iter(mats.values()))
+      width = self.group_width(gname)
+      concat = mat if mat.shape[1] == width else mat[:, :width]
+    else:
+      concat = torch.cat(per_feature, dim=1)
+    if reg is not None:
+      # the embedding regulariser covers what was LOOKED UP (the group's columns and the histories,
+      # input_layer.py:369-375, sequence_feature_layer.py:215-217), not the attended vectors appended to the concat
+      concat._er_reg = [v for v, k in zip(per_feature, kinds) if k == 'emb'] + reg
+    order = self.seqc_order.get(gname)
+    if order and len(order) > 1:
+      # the per-feature list keeps the sequence-combiner features in config order (the concat has them by name)
+      by_name = {e.name: v for e, v in zip(layout, per_feature) if e.kind == 'seqc'}
+      per_feature = [v for e, v in zip(layout, per_feature) if e.kind != 'seqc'] + [by_name[n] for n in order]
+    if gname in self.seq_group_layout:
+      seq, seq_len = self._seq_group_tensors(gname, features, outs_by_key)
+      # the embedding regulariser covers the un-pooled sequence embeddings and the plain embedding columns
+      # (input_layer.py:117-151, 176-191)
+      seq._er_reg = [seq] + [v for v, k in zip(per_feature, kinds) if k == 'emb']
+      return seq, seq_len, concat, per_feature
+    return concat, per_feature
 
   def _seq_group_tensors(self, gname, features, outs_by_key):
     """EnhancedInputLayer.build (layers/common_layers.py:114-127) with concat_seq_feature: the group's sequence
@@ -998,12 +1037,12 @@ class InputLayer(object):
     lay = self.seq_group_layout[gname]
     B, T = self.batch_size, lay['T']
     parts = []   # [matrix, first column, width]: neighbouring columns of one matrix are one view
-    for _, d, ok, c in lay['seq']:
-      mat = outs_by_key[(d, ok)]
-      if parts and parts[-1][0] is mat and parts[-1][1] + parts[-1][2] == c:
-        parts[-1][2] += d
+    for e in lay['seq']:
+      mat = outs_by_key[(e.dim, e.out_key)]
+      if parts and parts[-1][0] is mat and parts[-1][1] + parts[-1][2] == e.col:
+        parts[-1][2] += e.dim
       else:
-        parts.append([mat, c, d])
+        parts.append([mat, e.col, e.dim])
     views = [m[:, c:c + w].reshape(B, T, w) for m, c, w in parts]
     seq = views[0] if len(views) == 1 else torch.cat(views, dim=-1)
-    return seq, features['seq_fea'][lay['seq'][0][0]][1]
+    return seq, features['seq_fea'][lay['seq'][0].name][1]

@@ -28,7 +28,7 @@ class SimpleMultiTask(MMoE):
   def __init__(self, input_layer, group, towers, tower_units, l2_reg=0.0, embedding_reg=0.0, generator=None):
     nn.Module.__init__(self)
     self.input_layer, self.group = input_layer, group
-    self.in_dim = d = sum(e[2] for e in input_layer.group_layout[group])
+    self.in_dim = d = input_layer.group_width(group)
     self.tower_names = [t[0] for t in towers]
     self.label_names = [t[1] for t in towers]
     self.task_weights = [t[2] for t in towers]
@@ -66,7 +66,7 @@ class DBMTL(MMoE):
                l2_reg=0.0, embedding_reg=0.0, generator=None):
     nn.Module.__init__(self)
     self.input_layer, self.group = input_layer, group
-    self.in_dim = d = sum(e[2] for e in input_layer.group_layout[group])
+    self.in_dim = d = input_layer.group_width(group)
     self.tower_names = [t[0] for t in towers]
     self.label_names = [t[1] for t in towers]
     self.task_weights = [t[2] for t in towers]
@@ -132,7 +132,7 @@ class PLE(MMoE):
   def __init__(self, input_layer, group, towers, nets, tower_units, l2_reg=0.0, embedding_reg=0.0, generator=None):
     nn.Module.__init__(self)
     self.input_layer, self.group = input_layer, group
-    self.in_dim = d = sum(e[2] for e in input_layer.group_layout[group])
+    self.in_dim = d = input_layer.group_width(group)
     self.tower_names = [t[0] for t in towers]
     self.label_names = [t[1] for t in towers]
     self.task_weights = [t[2] for t in towers]

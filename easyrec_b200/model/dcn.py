@@ -27,7 +27,7 @@ class DCN(RankModel):
     super().__init__()
     self.input_layer = input_layer
     self.group = group
-    d = sum(e[2] for e in input_layer.group_layout[group])
+    d = input_layer.group_width(group)
     self.in_dim = d
     self.dnn = L.DNN(d, deep_units, generator=generator)
     lim = math.sqrt(6.0 / (d + d))  # glorot uniform of a [d] variable: fan_in = fan_out = d

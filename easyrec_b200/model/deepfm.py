@@ -33,14 +33,14 @@ class DeepFM(nn.Module):
                generator=None):
     super().__init__()
     for gname in ('wide', 'deep'):
-      if any(e[1] == 'att' for e in input_layer.group_layout.get(gname, [])):
+      if any(e.kind == 'att' for e in input_layer.group_layout.get(gname, [])):
         raise NotImplementedError('DeepFM over a group with sequence_features (the FM fields must share one width)')
     self.input_layer = input_layer
     deep_layout = input_layer.group_layout['deep']
     self.n_field = len(deep_layout)
-    self.dim = deep_layout[0][2]
+    self.dim = deep_layout[0].width
     # (a SequenceFeature pooled by its sequence_combiner is one more field of the same width, input_layer.py:312-347)
-    assert all(e[2] == self.dim and e[1] in ('emb', 'seqc') for e in deep_layout), \
+    assert all(e.width == self.dim and e.kind in ('emb', 'seqc') for e in deep_layout), \
         'FM needs every deep feature embedded with the same dim'
     self.deep_width = self.n_field * self.dim
     self.dnn = L.DNN(self.deep_width, dnn_units, generator=generator)

@@ -36,8 +36,8 @@ class DLRM(RankModel):
       raise ValueError('arch_interaction_op must be dot or cat, got %r' % op)
     self.input_layer = input_layer
     self.op, self.itself, self.with_dense = op, bool(itself), bool(with_dense)
-    self.sparse_dims = [e[2] for e in lay['sparse']]
-    d_dense = sum(e[2] for e in lay['dense'])
+    self.sparse_dims = [e.width for e in lay['sparse']]
+    d_dense = input_layer.group_width('dense')
     self.d_dense = d_dense
     self.bot_dnn = L.DNN(d_dense, bot_units, generator=generator)
     D = self.bot_dnn.out_dim

@@ -32,8 +32,8 @@ class DSSM(RankModel):
                listwise=True, item_id=None, l2_reg=0.0, embedding_reg=0.0, generator=None):
     super().__init__()
     self.input_layer = input_layer
-    du = sum(e[2] for e in input_layer.group_layout['user'])
-    di = sum(e[2] for e in input_layer.group_layout['item'])
+    du = input_layer.group_width('user')
+    di = input_layer.group_width('item')
     self.du, self.di = du, di
     self.user_dnn = L.DNN(du, user_units[:-1], generator=generator) if len(user_units) > 1 else nn.Identity()
     self.user_out = L.Dense(user_units[-2] if len(user_units) > 1 else du, user_units[-1], generator)

@@ -33,7 +33,7 @@ class MMoE(RankModel):
     self.input_layer = input_layer
     self.group = group
     self.backbone = backbone
-    d = backbone.out_dim if backbone is not None else sum(e[2] for e in input_layer.group_layout[group])
+    d = backbone.out_dim if backbone is not None else input_layer.group_width(group)
     self.in_dim = d
     self.experts = nn.ModuleList([L.DNN(d, u, generator=generator) for u in expert_units])
     h = self.experts[0].out_dim

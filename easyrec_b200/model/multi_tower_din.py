@@ -36,15 +36,15 @@ class MultiTowerDIN(RankModel):
     self.tower_dnn = nn.ModuleList()
     total = 0
     for g, units in towers:
-      d = sum(e[2] for e in input_layer.group_layout[g])
+      d = input_layer.group_width(g)
       self.tower_bn.append(L.BatchNorm(d))
       self.tower_dnn.append(L.DNN(d, units, generator=generator))
       total += self.tower_dnn[-1].out_dim
     self.din_dnn = nn.ModuleList()
     for g, units in din_towers:
       lay = input_layer.seq_layout[g]
-      dk = sum(e[1] for e in lay['key'])
-      dh = sum(e[1] for e in lay['hist'])
+      dk = sum(e.dim for e in lay['key'])
+      dh = sum(e.dim for e in lay['hist'])
       assert dk == dh, 'DIN key dim %d != history dim %d' % (dk, dh)
       self.din_dnn.append(L.DNN(4 * dh, units, last_layer_no_activation=True, last_layer_no_batch_norm=True,
                                 generator=generator))

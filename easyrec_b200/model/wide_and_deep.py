@@ -10,10 +10,6 @@ from easyrec_b200 import model as registry
 from easyrec_b200.model.rank_model import RankModel
 
 
-def _group_width(input_layer, name):
-  return sum(e[2] for e in input_layer.group_layout[name])
-
-
 def _sum_features(x, n_feature):
   """tf.add_n over the group's per-feature [B, w] outputs, read from the group's [B, n_feature * w] concat"""
   B = x.shape[0]
@@ -39,12 +35,12 @@ class WideAndDeep(RankModel):
     super().__init__()
     for gname in ('wide', 'deep'):
       assert input_layer.has_group(gname), 'WideAndDeep needs feature groups "wide" and "deep"'
-    if any(e[1] != 'emb' for e in input_layer.group_layout['wide']):
+    if any(e.kind != 'emb' for e in input_layer.group_layout['wide']):
       raise NotImplementedError('WideAndDeep: the wide group must hold embedded features only')
     self.input_layer = input_layer
     self.n_wide = len(input_layer.group_layout['wide'])
-    self.wide_dim = _group_width(input_layer, 'wide') // self.n_wide
-    self.dnn = L.DNN(_group_width(input_layer, 'deep'), dnn_units, generator=generator)
+    self.wide_dim = input_layer.group_width('wide') // self.n_wide
+    self.dnn = L.DNN(input_layer.group_width('deep'), dnn_units, generator=generator)
     self.final_dnn = None
     if final_units:
       self.final_dnn = L.DNN(self.wide_dim + self.dnn.out_dim, final_units, generator=generator)
@@ -80,10 +76,10 @@ class FM(RankModel):
   def __init__(self, input_layer, l2_reg=0.0, embedding_reg=0.0):
     super().__init__()
     lay = input_layer.group_layout['deep']
-    if any(e[1] != 'emb' for e in lay) or len({e[2] for e in lay}) != 1:
+    if any(e.kind != 'emb' for e in lay) or len({e.width for e in lay}) != 1:
       raise NotImplementedError('FM: the deep group must hold embedded features of one width')
     self.input_layer = input_layer
-    self.n_field, self.dim = len(lay), lay[0][2]
+    self.n_field, self.dim = len(lay), lay[0].width
     self.n_wide = len(input_layer.group_layout['wide'])
     self.fm_bias = nn.Parameter(torch.zeros(1))
     self.l2_reg, self.embedding_reg = l2_reg, embedding_reg

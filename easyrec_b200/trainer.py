@@ -303,7 +303,7 @@ class Trainer(object):
         # the gathered K7 reads the clip factor from the device-resident gradient scale (x 1/N, replica_grad_scale);
         # the dense buffer already holds the averaged, regularised, clipped gradient
         self.dp.apply_sparse(self._step_pending, self.input_layer.opt_holder['opt'])
-        self.input_layer._pending = []
+        self.input_layer.discard_pending()
         self.dense_opt.apply(l2_folded=True, grad_scale=1.0)
       else:
         self.input_layer.backward_update()
@@ -313,7 +313,7 @@ class Trainer(object):
       self.input_layer.backward_update()   # K7: dedup + fused row update, on this thread/stream
     elif self.dp.sparse:
       self.dp.apply_sparse(self._step_pending, self.input_layer.opt_holder['opt'])
-      self.input_layer._pending = []
+      self.input_layer.discard_pending()
     self.dense_opt.apply()                 # one launch: l2 + adagrad/adam over the flat buffer
     if self._ep_side is not None:
       torch.cuda.current_stream().wait_stream(self._ep_side)   # the row-sharded backward of _segment_exchange

@@ -535,7 +535,7 @@ def seqc_batch():
 def test_attention_sequence_combiner_in_a_plain_group(doubles):
   cfg = config_util.get_configs_from_pipeline_file(CFG_SEQC)
   il, model, _ = builder.build_model(cfg, 4, 'cpu', cpu_generator=torch.Generator().manual_seed(2))
-  assert [e[0] for e in il.group_layout['g']] == ['u', 'aa', 'zz']          # concat: plain features, then by name
+  assert [e.name for e in il.group_layout['g']] == ['u', 'aa', 'zz']          # concat: plain features, then by name
   assert il.seqc_order['g'] == ['zz', 'aa']                                  # per-feature list: config order
   with torch.no_grad():
     for m in il.attention_modules.values():
@@ -552,7 +552,7 @@ def test_attention_sequence_combiner_in_a_plain_group(doubles):
   assert len(reg) == 3 and sorted(tuple(r.shape) for r in reg) == [(4, 3, 4), (4, 3, 4), (4, 4)]
   want_sq = (u ** 2).sum() + (unpooled['aa'] ** 2).sum() + (unpooled['zz'] ** 2).sum()
   assert float(sum((r * r).sum() for r in reg)) == pytest.approx(float(want_sq), rel=1e-5)
-  il._pending = []
+  il.discard_pending()
   # ... and the whole thing trains: table rows, attention vectors and towers move, the loss falls
   from easyrec_b200.estimator import EasyRecEstimator
   est = EasyRecEstimator(CFG_SEQC, device='cpu', seed=2)

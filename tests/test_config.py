@@ -83,7 +83,7 @@ def test_config_to_table_plan_and_schedule():
   il, model, opt = builder.build_model(cfg, 32, 'cpu', cpu_generator=torch.Generator().manual_seed(0))
   assert set(il.arenas) == {16, 1}
   assert il.arenas[16].n_rows == 1 + 1000  # raw projection row + hashed table
-  assert [e[0] for e in il.group_layout['deep']] == ['F1', 'C1']  # config order
+  assert [e.name for e in il.group_layout['deep']] == ['F1', 'C1']  # config order
   assert opt['kind'] == 'adam_optimizer'
   lr = opt['lr_fn']
   assert abs(lr(0) - 0.001) < 1e-9 and abs(lr(999) - 0.001) < 1e-9   # staircase (proto floats are fp32)

@@ -529,7 +529,7 @@ def test_embed_test_seq_multi_embed_verbatim(tmp_path):
       so = il.seq_outputs['din']
       want = torch.tensor([[[2., 3.], [4., 5.], [0., 0.]], [[5., 6.], [7., 8.], [1., 2.]]])
       assert torch.allclose(so['hist_seq_emb'], want) and so['hist_seq_len'].tolist() == [2, 3]
-      il._pending = []
+      il.discard_pending()
   finally:
     mp.undo()
 

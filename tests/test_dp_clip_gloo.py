@@ -72,7 +72,7 @@ def _worker(rank, port, ret, world, cuda=False):
       ww = np.ones(rr.size, np.float32) if w is None else w.cpu().numpy()[lo:lo + rr.size]
       for u in np.unique(rr[rr >= 0]):
         local_sq += float(((g[rr == u] * ww[rr == u, None]).sum(0).astype(np.float64) ** 2).sum())
-  il._pending = []
+  il.discard_pending()
   tot = torch.tensor([local_sq], dtype=torch.float64, device=dev)
   dist.all_reduce(tot)
   g_avg = tr.dense_opt.flat_g.double().clone()
@@ -158,7 +158,7 @@ def _worker_ep(rank, port, ret, world, cuda=False):
       per_lookup[lo:lo + n] = g * ww[:, None]
     for u in np.unique(r[r >= 0]):
       local_sq += float((per_lookup[r == u].sum(0) ** 2).sum())
-  il._pending = []
+  il.discard_pending()
   tot = torch.tensor([local_sq], dtype=torch.float64, device=dev)
   dist.all_reduce(tot)
   g_avg = tr.dense_opt.flat_g.double().clone()

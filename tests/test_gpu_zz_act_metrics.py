@@ -182,7 +182,7 @@ model_config { model_class: "MultiTowerDIN"
   so = il.seq_outputs['din']
   want = torch.tensor([[[2., 3.], [4., 5.], [6., 7.], [8., 9.]], [[10., 11.], [0., 0.], [11., 12.], [0., 0.]]], device=DEV)
   assert torch.allclose(so['hist_seq_emb'], want, atol=1e-6) and so['hist_seq_len'].tolist() == [4, 3]
-  il._pending = []
+  il.discard_pending()
   before = t.weight[off:off + 6].clone()
   tr = Trainer(model, il, 'adagrad', lr=0.1)
   loss, _ = tr.train_step(feats, labels)
@@ -229,7 +229,7 @@ def test_attention_sequence_combiner_on_the_kernels():
   u, pooled, _ = seqc_expected(il, feats)
   np.testing.assert_allclose(concat.detach().cpu().numpy(), np.concatenate([u, pooled['aa'], pooled['zz']], 1), rtol=1e-5, atol=1e-6)
   np.testing.assert_allclose(per_feature[1].detach().cpu().numpy(), pooled['zz'], rtol=1e-5, atol=1e-6)
-  il._pending = []
+  il.discard_pending()
   w0 = [m.kernel.detach().clone() for m in il.attention_modules.values()]
   t0 = il.arenas[4].weight.clone()
   tr = Trainer(model, il, 'adagrad', lr=0.1)

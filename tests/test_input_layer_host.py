@@ -162,3 +162,37 @@ def test_reference_packed_batch_through_input_layer_matches_embedding_parallel_l
     feats = readers.from_reference_packed(il, {'sparse_fea': (np.array(rank['ids'], np.int64), np.array(rank['lens'], np.int32))}, names)
     deep, _ = il.lookup(feats)['deep']
     np.testing.assert_allclose(deep.detach().numpy()[:, :F * D], np.array(rank['y'], np.float32), rtol=1e-6, atol=1e-6)
+
+
+def test_every_column_reads_the_slot_it_was_planned_with(monkeypatch):
+  """Each layout column reads the ArenaCall column of its own slot.  The plan has one feature in two groups of the
+  same width, in-group sequence_features whose key is a plain column of the group, and a history listed twice (two
+  slots of one table, as a reference sample config has it): every one of them keeps its own slot's column."""
+  import collections
+  from easyrec_b200 import input_layer as IL
+  monkeypatch.setenv('ER_PLAN_ONLY', '1')
+  feats = [IL.id_feature('item', 8, hash_bucket_size=100), IL.id_feature('cate', 8, num_buckets=30),
+           IL.id_feature('user', 8, hash_bucket_size=50), IL.raw_feature('price', 8),
+           IL.multi_feature('hist', 'seq', 8, hash_bucket_size=100, seq_len=5)]
+  seq = [dict(name='att', maps=[(['cate'], ['hist']), (['cate'], ['hist'])], units=[4, 1], need_key=True)]
+  groups = collections.OrderedDict([('user', dict(features=['user', 'item', 'price'])),
+                                    ('item', dict(features=['price', 'item', 'cate'], seq=seq))])
+  seq_att = collections.OrderedDict([('din', [(['item'], ['hist'])])])
+  il = IL.InputLayer(feats, groups, 4, 'cpu', seq_att_groups=seq_att, dense_generator=torch.Generator().manual_seed(0))
+  col_of = {id(s): c for subs in il.subcalls.values() for sc in subs.values()
+            for s, c in zip(sc.call.slots, sc.call.slot_cols)}
+  columns = [e for lay in il.group_layout.values() for e in lay]
+  columns += [e for lay in il.seq_layout.values() for e in lay['key'] + lay['hist']]
+  looked_up = [e for e in columns if e.slot is not None]
+  assert len(looked_up) == 12 and all(e.slot is not None for e in columns if getattr(e, 'kind', None) == 'emb')
+  for e in looked_up:
+    assert e.slot.name == '%s/%s' % (e.out_key, e.name) and e.col == col_of[id(e.slot)], e
+  user, item = il.group_layout['user'], il.group_layout['item']
+  assert [(e.name, e.col) for e in user] == [('user', 0), ('item', 8), ('price', 16)]
+  assert [(e.name, e.col) for e in item[:3]] == [('price', 0), ('item', 8), ('cate', 16)]
+  assert user[1].slot is not item[1].slot and user[2].slot is not item[2].slot
+  att = il.seq_layout['item/att']
+  assert [e.slot for e in att['key']] == [item[2].slot] * 2 and [e.col for e in att['key']] == [16, 16]
+  assert [e.col for e in att['hist']] == [0, 8] and att['hist'][0].slot is not att['hist'][1].slot
+  assert item[3] == IL.GroupColumn('seq_fea/att', 'att', 32, out_key='item/att', need_key=True)
+  assert il.group_width('user') == 24 and il.group_width('item') == 56

@@ -473,7 +473,7 @@ model_config { model_class: "DeepFM"
   est.model.train()
   logits = est.model(feats).detach()
   want_loss, _, _ = O.sigmoid_ce(logits.numpy(), labels.numpy(), weights=feats['sample_weight'].numpy())
-  il._pending = []
+  il.discard_pending()
   loss, _ = est.trainer.train_step(feats, labels)
   reg = float(est.trainer.dense_opt.reg_loss[0])     # deepfm.l2_regularization defaults to 1e-4 (protos/deepfm.proto)
   assert abs(float(loss) - reg - want_loss) < 1e-6
@@ -537,7 +537,7 @@ def test_global_norm_clipping_scales_every_gradient_by_clip_over_the_tf_global_n
   got_sparse = float(il.sparse_grad_sqnorm())
   got = float(torch.sqrt(torch.tensor(got_sparse) + ((opt.flat_g + l2 * opt.flat_p) ** 2).sum()))
   assert got == pytest.approx(np.sqrt(want_sq), rel=1e-5)
-  il._pending = []
+  il.discard_pending()
   # -- the step: with plain SGD every update is linear in its gradient, so clipped = scale * unclipped everywhere
   clip2 = EasyRecEstimator(CLIP_CFG % b'gradient_clipping_by_norm: 0.05', device='cpu', seed=11)
   before_p = plain.trainer.dense_opt.flat_p.clone()
@@ -580,7 +580,7 @@ def test_l2_loss_types_train_the_rank_head_as_a_regressor(loss_type, dense_kerne
   loss, pred = est.model.loss(logits, labels)
   want = ((y - labels) ** 2).mean() + est.model.regularization_loss()
   assert abs(float(loss) - float(want)) < 1e-6 and torch.allclose(pred, y.detach())
-  est.input_layer._pending = []
+  est.input_layer.discard_pending()
   losses = [float(est.trainer.train_step(feats, labels)[0]) for _ in range(30)]
   assert losses[-1] < losses[0]
 
@@ -631,7 +631,7 @@ model_config { model_class: "MultiTower"
   cfg = config_util.get_configs_from_pipeline_file(text.encode())
   B = 256
   il, model, opt = builder.build_model(cfg, B, 'cpu', cpu_generator=torch.Generator().manual_seed(1), default_seq_len=20)
-  assert [e[1] for e in il.group_layout['item']] == ['emb', 'emb', 'emb', 'att'] and il.group_layout['item'][-1][2] == 32
+  assert [e.kind for e in il.group_layout['item']] == ['emb', 'emb', 'emb', 'att'] and il.group_layout['item'][-1].width == 32
   assert 'item' in il.arenas[16].tables and 'item_id_embedding' not in il.arenas[16].tables   # key and history share it
   assert sorted(dict(model.named_parameters())) != [] and any(n.startswith('input_attention.') for n, _ in model.named_parameters())
   rng = np.random.default_rng(0)
@@ -659,7 +659,7 @@ model_config { model_class: "MultiTower"
   want = O.din_attention(key, he.astype(np.float32), lens, layers)
   np.testing.assert_allclose(concat[:, 48:64].detach().numpy(), want, rtol=1e-4, atol=1e-6)
   assert len(concat._er_reg) == 4     # three looked-up columns + the history
-  il._pending = []
+  il.discard_pending()
   tr = T.Trainer(model, il, 'adagrad', lr_fn=opt['lr_fn'])
   lab = torch.from_numpy((rng.uniform(size=B) < 0.3).astype(np.float32))
   p0 = dnn.layers[0].kernel.detach().clone()
@@ -729,7 +729,7 @@ def test_wide_and_deep_and_fm_model_classes_match_their_formulas(interaction_dou
     logits = model(feats).detach()
     g = il.lookup(feats)
     wide, deep = g['wide'][0].detach(), g['deep'][0].detach()
-    il._pending = []
+    il.discard_pending()
     if name == 'FM':
       assert wide.shape == (B, 3)                                       # wide_output_dim = num_class = 1
       v = deep.reshape(B, 4, 16)
@@ -861,7 +861,7 @@ model_config { model_class: "RankModel"
       want_kv = (rows_k * wk[:, :, None]).sum(1) / wk.sum(1, keepdims=True)
     want_kv[2] = 0.0   # a sample without tags: the reference divides 0 by 0 there (NaN); this path gives the zero vector
     np.testing.assert_allclose(out[:, 12:18], want_kv, rtol=1e-5, atol=1e-7)
-    il._pending = []
+    il.discard_pending()
   tr = T.Trainer(model, il, 'adagrad', lr_fn=opt['lr_fn'])
   feats, labels = list(readers.CSVInput(cfg, il, str(tmp_path / 't.csv')))[0]
   losses = [float(tr.train_step(feats, labels)[0]) for _ in range(20)]
@@ -922,7 +922,7 @@ model_config { model_class: "MultiTower"
   assert any(s is not None for _, _, _, _, s in il._pending)       # the call really holds CSR slots
   got_sparse = float(il.sparse_grad_sqnorm())
   assert got_sparse == pytest.approx(want_sq, rel=1e-5) and want_sq > 0
-  il._pending = []
+  il.discard_pending()
   # -- the step: SGD, clipped = scale * unclipped on the table and the towers
   p0 = plain.trainer.dense_opt.flat_p.clone()
   t0 = {d: a.weight.clone() for d, a in plain.input_layer.arenas.items()}
