@@ -457,40 +457,44 @@ class InputLayer(object):
     self.seq_group_layout = {g: dict(lay, seq=resolved(lay['seq'])) for g, lay in self.seq_group_layout.items()}
 
   def _plan_exchanges(self):
-    """EmbeddingParallel: a ShardedLookup around every sub-call"""
+    """EmbeddingParallel: a ShardedLookup around every sub-call.  The single-valued and multi-valued (CSR) launches of
+    an arena form ONE exchange - one K8, one row update per table on the owner - shared by the arenas of the same
+    combined row plan (the wide dim-1 tables next to the deep ones); every history launch has an exchange of its own."""
     from easyrec_b200.sharded import ShardedLookup
     shard_n, shard_rank = self._shard
-    exchanges = {}   # row plan -> the exchange its arenas share (ids once, rows in one packed all-to-all)
+    exchanges = {}       # combined row plan -> the exchange its arenas share (ids once, rows in one packed all-to-all)
+    self._ex_plan = []   # (exchange, dim of its first arena, that arena's launches in range order)
     for dim, subs in self.subcalls.items():
       for sk, sc in subs.items():
-        if sc.kind != 'single':
-          # multi-valued slots (the ragged forms of embedding_parallel_lookup) and un-pooled histories (one lookup per
-          # step, padded steps dropped by K1): an exchange of their own.  The owner applies one row update per
-          # exchange, so a table must not be read by slots of two different launches
-          mine = set(slot.table for _, _, slot, _ in sc.items)
-          for sk2, sc2 in subs.items():
-            shared = sorted(mine & set(slot.table for _, _, slot, _ in sc2.items)) if sc2 is not sc else None
-            if shared and 'seq' in (sc.kind, sc2.kind):
-              raise NotImplementedError('EmbeddingParallel: table(s) %s are read both by history (SequenceFeature) '
-                                        'steps and by other features; give the histories tables of their own'
-                                        % shared)
-            if shared:
-              raise NotImplementedError('EmbeddingParallel: table(s) %s are shared by single- and multi-valued features'
-                                        % shared)
-          if sc.kind == 'seq' and len(subs) > 1 and self.arenas[dim].opt_kind == _lib.OPT_ADAM_ROWS:
-            # adam_optimizer's dense decay sweeps every row the owner did not update: with two exchanges on one arena
-            # each would sweep the rows only the other one updated
-            raise NotImplementedError('EmbeddingParallel: adam_optimizer with histories next to other features of '
-                                      'embedding_dim %d (their tables share one arena and two exchanges)' % dim)
-          seq = (self.batch_size, sk[1]) if sc.kind == 'seq' else None
-          sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, seq=seq)
-          if len(subs) == 1:
-            self.merged[dim].sharded = sc.sharded
+        if sc.kind != 'seq':
           continue
-        key = self._rows_key(sc)
-        sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, exchange=exchanges.get(key))
-        exchanges.setdefault(key, sc.sharded.ex)
-        self.merged[dim].sharded = sc.sharded
+        # un-pooled histories (one lookup per step, padded steps dropped by K1): an exchange of their own.  The owner
+        # applies one row update per exchange, so a table must not be read by a history and by another launch
+        mine = set(slot.table for _, _, slot, _ in sc.items)
+        for sk2, sc2 in subs.items():
+          shared = sorted(mine & set(slot.table for _, _, slot, _ in sc2.items)) if sc2 is not sc else None
+          if shared:
+            raise NotImplementedError('EmbeddingParallel: table(s) %s are read both by history (SequenceFeature) '
+                                      'steps and by other features; give the histories tables of their own'
+                                      % shared)
+        if len(subs) > 1 and self.arenas[dim].opt_kind == _lib.OPT_ADAM_ROWS:
+          # adam_optimizer's dense decay sweeps every row the owner did not update: with two exchanges on one arena
+          # each would sweep the rows only the other one updated
+          raise NotImplementedError('EmbeddingParallel: adam_optimizer with histories next to other features of '
+                                    'embedding_dim %d (their tables share one arena and two exchanges)' % dim)
+        sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, seq=(self.batch_size, sk[1]))
+      flat = [sc for sc in subs.values() if sc.kind != 'seq']
+      if flat:
+        key = tuple(self._rows_key(sc) for sc in flat)
+        ex = exchanges.get(key)
+        for sc in flat:
+          sc.sharded = ShardedLookup(sc.call, shard_n, shard_rank, exchange=ex)
+          ex = sc.sharded.ex
+        if key not in exchanges:
+          exchanges[key] = ex
+          self._ex_plan.append((ex, dim, flat))
+      if len(subs) == 1:
+        self.merged[dim].sharded = next(iter(subs.values())).sharded
 
   def group_width(self, name):
     """width of the group's concat [B, width]"""
@@ -563,11 +567,17 @@ class InputLayer(object):
 
   def check_exchange(self):
     """EmbeddingParallel: raise if a per-peer block of the fixed-capacity exchange overflowed since the last check
-    (reads one counter per arena back: call it outside the step loop, e.g. when the loss is logged)."""
-    if self.ep:
-      for subs in self.subcalls.values():
-        for sc in subs.values():
-          sc.sharded.check()
+    (reads one counter per arena back: call it outside the step loop, e.g. when the loss is logged), or if a prefetched
+    batch was not the one looked up.  Every exchange's counters are read and reset before the first error is raised."""
+    err = None
+    for ex in self._exchanges():
+      ex.build()
+      try:
+        ex.check()
+      except _lib.ErError as e:
+        err = err or e
+    if err is not None:
+      raise err
 
   def sparse_grad_sqnorm(self):
     """sum over the tables of ||IndexedSlices.values||^2 as TF would build them after loss.backward(): the gradient of a
@@ -666,23 +676,12 @@ class InputLayer(object):
 
   def prefetch_exchange(self, next_features):
     """EmbeddingParallel: start the id half of the NEXT batch's exchange (K1, K8, id all-to-all) beside the rest of
-    this step; the next lookup() promotes it instead of computing it on the critical path."""
+    this step; the next lookup() promotes it instead of computing it on the critical path.  (The histories' exchanges
+    run with their lookup.)"""
     if not self.ep:
       return
-    done = set()
-    for dim, subs in self.subcalls.items():
-      for sk, sc in subs.items():
-        if sc.kind != 'single':
-          continue                 # (variable-length inputs: their id exchange runs with the lookup)
-        ex = sc.sharded.ex
-        if id(ex) in done:
-          continue
-        done.add(id(ex))
-        buf = self._next_ids.get(dim)
-        if buf is None:
-          buf = self._next_ids[dim] = torch.zeros_like(self.static_ids[dim])
-        cids, _ = self._gather_inputs(dim, next_features.get('sparse_fea'), None, ids_buf=buf, want_w=False)
-        ex.prefetch(ex.members[0], cids)
+    for ex, dim, flat in self._ex_plan:
+      ex.prefetch(lambda: self._exchange_inputs(dim, flat, next_features, None, prefetch=True))
 
   def _exchanges(self):
     seen, out = set(), []
@@ -758,31 +757,67 @@ class InputLayer(object):
   # ------------------------------------------------------------------
   @staticmethod
   def _rows_key(sc):
+    """what decides the rows a launch looks up: its slots' bucket rules and offsets and where its ids come from (a
+    multi-valued launch: its kind, its features and its lookup capacity too, and which of its slots K1 prunes by
+    weight - a weighted mean / sqrtn lookup whose weight is not > 0 reads no row, a sum lookup keeps it, so a mean
+    TagFeature in a deep group and its sum twin in a wide group look up different rows)"""
     key = getattr(sc, 'rows_key', None)
     if key is None:
       call = sc.call
       key = (tuple((int(r['num_buckets']), int(r['row_offset']), int(r['seg_begin']), int(r['n_seg']),
-                    int(r['bucket_mode']), int(r['shard_n'])) for r in call.slots_np), tuple(call.sources))
+                    int(r['bucket_mode']), int(r['shard_n'])) for r in call.slots_np),
+             tuple(call.sources) if sc.kind == 'single' else (sc.kind, call.max_lookups) + tuple(
+                 src for _, _, _, src in sc.items) + tuple(
+                 (int(r['combiner']) & 0xf) != _lib.COMBINER_SUM for r in call.slots_np))
       sc.rows_key = key
     return key
+
+  def _exchange_inputs(self, dim, flat, features, dense_norm, prefetch=False):
+    """[LaunchInput] of an exchange's launches `flat` (those of its first arena, `dim`) for the batch `features`, and
+    the pooling inputs of each: [(weights, row_ptr, seg_ids)]"""
+    from easyrec_b200.sharded import LaunchInput
+    parts, pool = [], []
+    for sc in flat:
+      if sc.kind == 'single':
+        if prefetch:
+          buf = self._next_ids.get(dim)
+          if buf is None:
+            buf = self._next_ids[dim] = torch.zeros_like(self.static_ids[dim])
+          cids, w = self._gather_inputs(dim, features.get('sparse_fea'), None, ids_buf=buf, want_w=False)
+        else:
+          cids, w = self._gather_inputs(dim, features.get('sparse_fea'), dense_norm)
+        parts.append(LaunchInput(cids))
+        pool.append((w, None, None))
+        continue
+      ids_cap, lens, weights = self._csr_inputs(sc, features)
+      row_ptr, seg_ids = K.csr_from_lens(lens.contiguous(), sc.call.max_lookups)
+      parts.append(LaunchInput(ids_cap, seg_ids, row_ptr, weights))
+      pool.append((weights, row_ptr, seg_ids))
+    return parts if prefetch else (parts, pool)
 
   def _run_subcall(self, dim, sk, sc, features, dense_norm):
     """K1 + K2 of one uniform launch; returns (rows, weights, row_ptr, seg_ids, outs)."""
     call = sc.call
     B = self.batch_size
+    if self.ep and sc.kind != 'seq':
+      # row-sharded tables: the first launch of an exchange this step runs K1 of all its launches, K8 and the
+      # all-to-alls for every arena of its row plan; each launch then pools the received rows by its own plan
+      ex = sc.sharded.ex
+      hit = self._ex_inputs.get(id(ex))
+      if hit is None:
+        _, dim0, flat = next(e for e in self._ex_plan if e[0] is ex)
+        parts, hit = self._exchange_inputs(dim0, flat, features, dense_norm)
+        ex.build()
+        ex.lookup(parts)
+        self._ex_inputs[id(ex)] = hit
+      w, row_ptr, seg_ids = hit[ex.launches.index(sc.sharded.ref)]
+      outs = call.alloc_outputs()
+      rows = sc.sharded.forward(None, w, outs, row_ptr=row_ptr, seg_ids=seg_ids)
+      for o in outs:
+        o.requires_grad_(True)
+      return rows, w, row_ptr, seg_ids, outs
     if sc.kind == 'single':
       key = self._rows_key(sc)   # arenas with the same row plan (wide dim-1 next to the deep tables) share K1's rows
-      if self.ep:
-        # ... and under EmbeddingParallel the whole exchange: the first arena of a row plan runs it for all of them
-        hit = self._rows_cache.get(key)
-        cids, w = (None, hit[1]) if hit is not None else self._gather_inputs(dim, features.get('sparse_fea'), dense_norm)
-        outs = call.alloc_outputs()
-        rows = sc.sharded.forward(cids, w, outs)
-        if hit is None:
-          self._rows_cache[key] = (rows, w)
-        for o in outs:
-          o.requires_grad_(True)
-        return rows, w, None, None, outs
       hit = self._rows_cache.get(key)
       if hit is None:
         cids, w = self._gather_inputs(dim, features.get('sparse_fea'), dense_norm)
@@ -825,13 +860,6 @@ class InputLayer(object):
     cap = call.max_lookups
     ids_cap, lens, weights = self._csr_inputs(sc, features)
     row_ptr, seg_ids = K.csr_from_lens(lens.contiguous(), cap)
-    if self.ep:
-      # row-sharded tables: K1 (owner, local row) -> K8 -> all-to-alls -> pooling of the received rows by the same CSR
-      outs = call.alloc_outputs()
-      rows = sc.sharded.forward(ids_cap, weights, outs, row_ptr=row_ptr, seg_ids=seg_ids)
-      for o in outs:
-        o.requires_grad_(True)
-      return rows, weights, row_ptr, seg_ids, outs
     rows = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
     K.bucketize(ids_cap, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr,
                 rows=rows, **K.k1_weight_args(ids_cap, weights))
@@ -908,6 +936,7 @@ class InputLayer(object):
     dense_norm = self.normalize_dense(dense) if dense is not None else None
     self._rows_cache = dict(self._preset_rows)   # K1 results computed ahead of the step (precompute_rows)
     self._preset_rows = {}
+    self._ex_inputs = {}   # EmbeddingParallel: exchange -> its launches' pooling inputs, once it ran for this batch
     self._pending = []
     outs_by_key = {}
     for dim, subs in self.subcalls.items():
@@ -936,7 +965,8 @@ class InputLayer(object):
     """the Pending K7 update(s) of one arena's launches `parts` [(sub-call, rows, weights, seg_ids, outs)]: several
     launches are packed into the arena's MergedCall"""
     if self.ep and len(parts) > 1:
-      # row-sharded tables: every launch has its own exchange and its own owner-side update (disjoint tables)
+      # row-sharded tables: every launch adds its gradient sums to its exchange; the exchange's last launch runs the
+      # owner-side updates
       for sc, rows, w, seg_ids, outs in parts:
         self._pending.append(Pending(sc, rows, w, outs, seg_ids))
     elif len(parts) == 1:
