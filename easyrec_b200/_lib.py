@@ -52,6 +52,12 @@ class ErBnStats(ctypes.Structure):
               ('moving_var', c_vp), ('eps', c_f32), ('momentum', c_f32)]
 
 
+class ErGemmPlane(ctypes.Structure):
+  """er_gemm_plane_t."""
+  _fields_ = [('src', c_vp), ('ld_row', c_i64), ('ld_k', c_i64), ('rows', c_i64), ('k', c_i64), ('hi', c_vp),
+              ('lo', c_vp)]
+
+
 class ErCsvCol(ctypes.Structure):
   """er_csv_col_t."""
   _fields_ = [('kind', c_i32), ('width', c_i32), ('inner_sep', ctypes.c_char), ('kv_sep', ctypes.c_char), ('pad_', ctypes.c_char * 6),
@@ -146,6 +152,10 @@ SIGNATURES = {
     'er_fm_block_fwd': (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp, c_sz, c_vp]),
     'er_fm_block_bwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_f32, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i32,
                                 c_vp]),
+    'er_gemm_plane_floats': (c_sz, [c_i64, c_i64]),
+    'er_gemm_split_planes': (c_i32, [ctypes.POINTER(ErGemmPlane), c_i32, c_vp]),
+    'er_gemm_planes': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
+                               ctypes.POINTER(ErBnStats), c_vp, c_sz, c_vp]),
     'er_gemm_workspace_bytes': (c_sz, [c_i64, c_i64, c_i64]),
     'er_gemm': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_i64, c_i32, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
                         c_vp, c_sz, c_vp]),

@@ -31,9 +31,17 @@
 // for 128 columns of tensor-core work.
 // Split-K partials are reduced by a second kernel in a fixed order: results are run-to-run deterministic.
 // The kernel is launched with programmatic dependent launch: its prologue overlaps the previous kernel's drain.
+//
+// Pre-split B (er_gemm_planes): the dense towers' weights change once per step but every 128-row tile of a forward or
+// dX GEMM would split (and, in forward, transpose) the same weight tiles again.  er_gemm_split_planes writes each
+// weight once per step as hi / lo planes in the exact K-major SWIZZLE_128B byte order of a B stage, zero-padded to
+// whole tiles ([row tile][k-block][NM rows][32 k]); the GEMM then fills a stage's B half with two bulk asynchronous
+// copies (cp.async.bulk, completed on the stage's mbarrier) issued by one thread, and the threads only stage A.  The
+// planes hold the bits the in-kernel split produces and the wgmma sequence is unchanged: results are bit-identical.
 #include <algorithm>
 
 #include "common.cuh"
+#include "tf32_split.cuh"
 
 namespace er {
 namespace gemm {
@@ -41,12 +49,13 @@ namespace gemm {
 constexpr int BM = 128, BN = 128, BK = 32;
 constexpr int kStages = 3;
 constexpr int kPrefetch = 2;      // k-blocks of global loads in flight per thread
+constexpr int kPrefetchPre = 3;   // the same with a pre-split B (only A goes through registers)
 constexpr int kThreads = 256;     // 2 warpgroups
 constexpr int kTileBytes = 128 * 128;          // 128 rows x 128 B
 constexpr int kStageBytes = 4 * kTileBytes;    // A hi, A lo, B hi, B lo
 constexpr int kOutPitch = BN + 8;              // floats per row of the staged output tile (conflict-free float2)
 constexpr int kStatFloats = 768;               // per-half Welford partials [2][128][3]; reused by the final merge
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* align slack */ + kStatFloats * 4 + 16;
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* align slack */ + kStatFloats * 4 + 16 + kStages * 8;
 static_assert(BM * kOutPitch * 4 <= kStages * kStageBytes, "output tile must fit in the stage ring");
 
 struct Args {
@@ -58,6 +67,10 @@ struct Args {
   long long lda, ldb, ldc;
   int M, N, K;
   int a_mn, b_mn;      // 1: the M (resp. N) index is the contiguous one in memory
+  // pre-split B planes (er_gemm_planes): hi / lo, plane_tile_floats(N, K) floats per 128-row tile; B is unused
+  const float* b_hi;
+  const float* b_lo;
+  long long b_tile_floats;
   int k_per_slice;     // multiple of BK
   int n_slices;
   // batch-norm statistics of the output columns (training forward of a dense+BN layer), optional
@@ -66,8 +79,34 @@ struct Args {
   er_bn_stats_t bn;
 };
 
+// MMA width of an N-column output (= rows of its B operand): the narrowest of 16/32/64/128 that covers N; wider
+// outputs are cut into 128-column tiles.
+__host__ __device__ constexpr int mma_width(long long n) { return n > 64 ? 128 : n > 32 ? 64 : n > 16 ? 32 : 16; }
+// floats of one 128-row tile of a pre-split plane of a [rows x K] K-major operand: ceil(K / BK) k-blocks of NM x BK
+__host__ __device__ constexpr long long plane_tile_floats(long long rows, long long k) {
+  return (k + BK - 1) / BK * mma_width(rows) * BK;
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n.reg .pred p;\nWAIT_%=:\n"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      "@!p bra WAIT_%=;\n}\n" ::"r"(bar), "r"(parity) : "memory");
+}
+// global -> shared bulk copy (bytes % 16 == 0, both ends 16 B aligned), completing `bytes` transactions on bar
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
 // wgmma shared-memory matrix descriptor of a K-major SWIZZLE_128B tile: 8-row groups 1024 B apart (SBO),
@@ -147,12 +186,6 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t
       : "l"(da), "l"(db), "r"(1));
 }
 
-__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
-  uint32_t h = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;  // round-to-nearest onto 10 mantissa bits
-  hi = __uint_as_float(h);
-  lo = x - hi;
-}
-
 __device__ __forceinline__ float4 mask_chunk(float4 v, int nvalid) {
   if (nvalid < 4) {
     if (nvalid < 1) v.x = 0.f;
@@ -225,15 +258,17 @@ __device__ __forceinline__ void wf_merge(Welford& a, const Welford& b) {   // Ch
   a.n = n;
 }
 
-template <int NM>
+template <int NM, bool kPreB>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tf32x3_kernel(Args a) {
   constexpr int R = NM / 2;   // accumulator registers per thread
+  constexpr int kPf = kPreB ? kPrefetchPre : kPrefetch;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_u32 = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;   // SWIZZLE_128B atoms: 1024 B aligned
   uint8_t* base_ptr = smem_raw + (smem_base - raw_u32);
   float* s_stats = reinterpret_cast<float*>(base_ptr + kStages * kStageBytes);
   int* s_flag = reinterpret_cast<int*>(s_stats + kStatFloats);
+  const uint32_t s_bar = smem_u32(s_flag + 4);   // kStages mbarriers: the pre-split B half of each stage has landed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
@@ -249,15 +284,16 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tf32x3_kernel(Args a) {
   }
   // kPrefetch k-blocks of global loads stay in flight per thread (register ring) so the HBM/L2 latency is paid
   // once per tile, not once per k-block.
-  float4 va[kPrefetch][4], vb[kPrefetch][4];
+  float4 va[kPf][4], vb[kPreB ? 1 : kPf][4];
   auto issue = [&](int kb, float4 (&xa)[4], float4 (&xb)[4]) {
     const int k0 = k_begin + kb * BK;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       xa[j] = load_pos(a.A, a.lda, a.a_mn, pa[j], m0, a.M, k0, k_end);
       // B rows past the MMA width are never read by the tensor core
-      xb[j] = pb[j].mn < NM ? load_pos(a.B, a.ldb, a.b_mn, pb[j], n0, a.N, k0, k_end)
-                            : make_float4(0.f, 0.f, 0.f, 0.f);
+      if constexpr (!kPreB)
+        xb[j] = pb[j].mn < NM ? load_pos(a.B, a.ldb, a.b_mn, pb[j], n0, a.N, k0, k_end)
+                              : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   };
   auto stage_out = [&](int kb, const float4 (&xa)[4], const float4 (&xb)[4]) {
@@ -266,29 +302,52 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tf32x3_kernel(Args a) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       store_pos(st, a.a_mn, pa[j], mask_chunk(xa[j], pos_nvalid(a.a_mn, pa[j], m0, a.M, k0, k_end)));
-      if (pb[j].mn < NM)
+      if (!kPreB && pb[j].mn < NM)
         store_pos(st + 2 * kTileBytes, a.b_mn, pb[j], mask_chunk(xb[j], pos_nvalid(a.b_mn, pb[j], n0, a.N, k0, k_end)));
     }
   };
+  // pre-split B: k-block kb's two planes -> stage kb % kStages (thread 0; the stage's previous wgmma's have retired)
+  auto issue_b = [&](int kb) {
+    constexpr uint32_t kPlaneBytes = NM * BK * 4;
+    const uint32_t st = smem_base + (uint32_t)(kb % kStages) * kStageBytes + 2 * kTileBytes;
+    const uint32_t bar = s_bar + 8u * (uint32_t)(kb % kStages);
+    const long long off = (long long)blockIdx.x * a.b_tile_floats + (long long)(k_begin / BK + kb) * (NM * BK);
+    mbar_expect_tx(bar, 2 * kPlaneBytes);
+    bulk_g2s(st, a.b_hi + off, kPlaneBytes, bar);
+    bulk_g2s(st + kTileBytes, a.b_lo + off, kPlaneBytes, bar);
+  };
+  if constexpr (kPreB) {
+    if (tid == 0) {
+      for (int s = 0; s < kStages; ++s) mbar_init(s_bar + 8u * s, 1);
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+  }
 
   float acc[R], acc2[R];
 #pragma unroll
   for (int i = 0; i < R; ++i) acc[i] = acc2[i] = 0.f;
 
   er_pdl_wait();
+  if (kPreB && tid == 0 && n_kb > 0) issue_b(0);
 #pragma unroll
-  for (int u = 0; u < kPrefetch; ++u)
-    if (u < n_kb) issue(u, va[u], vb[u]);
+  for (int u = 0; u < kPf; ++u)
+    if (u < n_kb) issue(u, va[u], vb[kPreB ? 0 : u]);
 
-  for (int kb0 = 0; kb0 < n_kb; kb0 += kPrefetch) {
+  for (int kb0 = 0; kb0 < n_kb; kb0 += kPf) {
 #pragma unroll
-    for (int u = 0; u < kPrefetch; ++u) {
+    for (int u = 0; u < kPf; ++u) {
       const int kb = kb0 + u;
       if (kb < n_kb) {
-        stage_out(kb, va[u], vb[u]);
-        if (kb + kPrefetch < n_kb) issue(kb + kPrefetch, va[u], vb[u]);
+        stage_out(kb, va[u], vb[kPreB ? 0 : u]);
+        if (kb + kPf < n_kb) issue(kb + kPf, va[u], vb[kPreB ? 0 : u]);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> tensor core
         __syncthreads();
+        if constexpr (kPreB) {
+          // past this barrier both warpgroups have retired the wgmma's of k-block kb - 2: its stage takes kb + 1
+          if (tid == 0 && kb + 1 < n_kb) issue_b(kb + 1);
+          mbar_wait(s_bar + 8u * (uint32_t)(kb % kStages), (uint32_t)(kb / kStages) & 1u);
+        }
         const uint32_t st = smem_base + (uint32_t)(kb % kStages) * kStageBytes;
         const uint32_t a_hi = st + (uint32_t)wg * (64u * 128u), b_hi = st + 2 * kTileBytes;
         fence_regs(acc);
@@ -478,17 +537,55 @@ static void plan(int64_t M, int64_t N, int64_t K, int* n_slices, int* k_per_slic
   *n_slices = (int)ceil_div(kblocks, per);
 }
 
-template <int NM>
+template <int NM, bool kPreB>
 static int launch(const Args& a, dim3 grid, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<NM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_tf32x3_kernel<NM, kPreB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          kSmemBytes);
     if (e != cudaSuccess) return er::fail(ER_ERR_CUDA, std::string("er_gemm: ") + cudaGetErrorString(e));
     attr_set = true;
   }
-  er::launch_pdl(gemm_tf32x3_kernel<NM>, grid, dim3(kThreads), (size_t)kSmemBytes, st, a);
+  er::launch_pdl(gemm_tf32x3_kernel<NM, kPreB>, grid, dim3(kThreads), (size_t)kSmemBytes, st, a);
   return ER_OK;
+}
+template <bool kPreB>
+static int launch_width(const Args& a, dim3 grid, cudaStream_t st) {
+  switch (mma_width(a.N)) {
+    case 128: return launch<128, kPreB>(a, grid, st);
+    case 64: return launch<64, kPreB>(a, grid, st);
+    case 32: return launch<32, kPreB>(a, grid, st);
+    default: return launch<16, kPreB>(a, grid, st);
+  }
+}
+
+// One thread per 16 B chunk of a plane pair: chunk c of row r of k-block kb holds the 4 k's of swizzle slot
+// c ^ (r % 8); elements past the operand's rows / K are zeros (what mask_chunk gives the in-kernel split).
+constexpr int kMaxPlaneJobs = 32;
+struct PlaneJobs {
+  er_gemm_plane_t j[kMaxPlaneJobs];
+};
+__global__ void split_planes_kernel(PlaneJobs jobs) {
+  const er_gemm_plane_t p = jobs.j[blockIdx.y];
+  const int nm = mma_width(p.rows);
+  const long long n_kb = (p.k + BK - 1) / BK;
+  const long long chunks = (p.rows + BN - 1) / BN * n_kb * nm * (BK / 4);
+  er_pdl_wait();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < chunks; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i & 7);
+    const long long rk = i >> 3;                  // (tile, kb, r) row of 32 k
+    const int r = (int)(rk % nm);
+    const long long tkb = rk / nm;
+    const long long row = tkb / n_kb * nm + r, k0 = tkb % n_kb * BK + 4 * (c ^ (r & 7));
+    float v[4], hi[4], lo[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      v[e] = row < p.rows && k0 + e < p.k ? p.src[row * p.ld_row + (k0 + e) * p.ld_k] : 0.f;
+      split_tf32(v[e], hi[e], lo[e]);
+    }
+    reinterpret_cast<float4*>(p.hi)[i] = make_float4(hi[0], hi[1], hi[2], hi[3]);
+    reinterpret_cast<float4*>(p.lo)[i] = make_float4(lo[0], lo[1], lo[2], lo[3]);
+  }
 }
 
 }  // namespace gemm
@@ -502,20 +599,25 @@ extern "C" size_t er_gemm_workspace_bytes(int64_t M, int64_t N, int64_t K) {
 
 extern "C" size_t er_gemm_bn_workspace_bytes(int64_t M, int64_t N);
 
+// B is given either in memory (B, ldb, b_mn_major) or as pre-split planes (b_hi, b_lo; B NULL)
 static int gemm_impl(const float* A, int64_t lda, int32_t a_mn_major, const float* B, int64_t ldb,
-                     int32_t b_mn_major, const float* bias, float* C, int64_t ldc, int64_t M, int64_t N,
-                     int64_t K, const er_bn_stats_t* bn, void* ws, size_t ws_bytes, er_stream_t stream) {
+                     int32_t b_mn_major, const float* b_hi, const float* b_lo, const float* bias, float* C,
+                     int64_t ldc, int64_t M, int64_t N, int64_t K, const er_bn_stats_t* bn, void* ws,
+                     size_t ws_bytes, er_stream_t stream) {
   using namespace er::gemm;
-  ER_REQUIRE(A && B && C, "null operand");
+  const bool pre_b = B == nullptr;
+  ER_REQUIRE(A && C && (pre_b ? b_hi && b_lo : true), "null operand");
   ER_REQUIRE(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "bad shape");
-  ER_REQUIRE((lda & 3) == 0 && (ldb & 3) == 0, "operand pitch must be a multiple of 4 floats");
-  ER_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
+  ER_REQUIRE((lda & 3) == 0 && (pre_b || (ldb & 3) == 0), "operand pitch must be a multiple of 4 floats");
+  ER_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(b_hi) & 15) == 0 && (reinterpret_cast<uintptr_t>(b_lo) & 15) == 0,
              "operands must be 16-byte aligned");
   // a pitch shorter than the row would read the next row's first elements as this row's last ones
-  ER_REQUIRE(lda >= (a_mn_major ? M : K) && ldb >= (b_mn_major ? N : K), "pitch smaller than row");
+  ER_REQUIRE(lda >= (a_mn_major ? M : K) && (pre_b || ldb >= (b_mn_major ? N : K)), "pitch smaller than row");
   ER_REQUIRE(ldc >= N, "ldc < N");
   Args a;
   a.A = A; a.B = B; a.C = C; a.bias = bias;
+  a.b_hi = b_hi; a.b_lo = b_lo; a.b_tile_floats = plane_tile_floats(N, K);
   a.lda = lda; a.ldb = ldb; a.ldc = ldc;
   a.M = (int)M; a.N = (int)N; a.K = (int)K;
   a.a_mn = a_mn_major ? 1 : 0; a.b_mn = b_mn_major ? 1 : 0;
@@ -538,9 +640,7 @@ static int gemm_impl(const float* A, int64_t lda, int32_t a_mn_major, const floa
   }
   cudaStream_t st = er::as_stream(stream);
   dim3 grid((unsigned)er::ceil_div(N, BN), (unsigned)er::ceil_div(M, BM), (unsigned)a.n_slices);
-  // MMA width: the narrowest of 16/32/64/128 columns that covers N (N > 128: every tile is 128 wide)
-  const int rc = N > 64 ? launch<128>(a, grid, st) : N > 32 ? launch<64>(a, grid, st)
-               : N > 16 ? launch<32>(a, grid, st) : launch<16>(a, grid, st);
+  const int rc = pre_b ? launch_width<true>(a, grid, st) : launch_width<false>(a, grid, st);
   if (rc != ER_OK) return rc;
   int launches = 1;
   if (a.n_slices > 1) {
@@ -558,7 +658,9 @@ static int gemm_impl(const float* A, int64_t lda, int32_t a_mn_major, const floa
 extern "C" int er_gemm(const float* A, int64_t lda, int32_t a_mn_major, const float* B, int64_t ldb,
                        int32_t b_mn_major, const float* bias, float* C, int64_t ldc, int64_t M, int64_t N,
                        int64_t K, void* ws, size_t ws_bytes, er_stream_t stream) {
-  return gemm_impl(A, lda, a_mn_major, B, ldb, b_mn_major, bias, C, ldc, M, N, K, nullptr, ws, ws_bytes, stream);
+  ER_REQUIRE(B, "null operand");
+  return gemm_impl(A, lda, a_mn_major, B, ldb, b_mn_major, nullptr, nullptr, bias, C, ldc, M, N, K, nullptr, ws,
+                   ws_bytes, stream);
 }
 
 extern "C" size_t er_gemm_bn_workspace_bytes(int64_t M, int64_t N) {
@@ -570,5 +672,47 @@ extern "C" int er_gemm_bn(const float* A, int64_t lda, int32_t a_mn_major, const
                           const er_bn_stats_t* bn, void* ws, size_t ws_bytes, er_stream_t stream) {
   if (!bn) return er::fail(ER_ERR_INVALID_ARG, "er_gemm_bn: bn is NULL");
   if (er::ceil_div(N, er::gemm::BN) > 256) return er::fail(ER_ERR_INVALID_ARG, "er_gemm_bn: N too large");
-  return gemm_impl(A, lda, a_mn_major, B, ldb, b_mn_major, nullptr, C, ldc, M, N, K, bn, ws, ws_bytes, stream);
+  ER_REQUIRE(B, "null operand");
+  return gemm_impl(A, lda, a_mn_major, B, ldb, b_mn_major, nullptr, nullptr, nullptr, C, ldc, M, N, K, bn, ws,
+                   ws_bytes, stream);
+}
+
+extern "C" size_t er_gemm_plane_floats(int64_t rows, int64_t K) {
+  if (rows <= 0 || K <= 0) return 0;
+  return (size_t)er::ceil_div(rows, (int64_t)er::gemm::BN) * (size_t)er::gemm::plane_tile_floats(rows, K);
+}
+
+extern "C" int er_gemm_split_planes(const er_gemm_plane_t* planes, int32_t n, er_stream_t stream) {
+  using namespace er::gemm;
+  ER_REQUIRE(n >= 0 && (n == 0 || planes), "bad plane list");
+  cudaStream_t st = er::as_stream(stream);
+  int launches = 0;
+  for (int i0 = 0; i0 < n; i0 += kMaxPlaneJobs) {
+    PlaneJobs jobs;
+    const int cnt = std::min(kMaxPlaneJobs, n - i0);
+    long long max_chunks = 0;
+    for (int i = 0; i < cnt; ++i) {
+      const er_gemm_plane_t& p = planes[i0 + i];
+      ER_REQUIRE(p.src && p.hi && p.lo, "null plane pointer");
+      ER_REQUIRE(p.rows > 0 && p.k > 0 && p.rows < (1ll << 31) && p.k < (1ll << 31), "bad plane shape");
+      ER_REQUIRE((reinterpret_cast<uintptr_t>(p.hi) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.lo) & 15) == 0,
+                 "planes must be 16-byte aligned");
+      jobs.j[i] = p;
+      max_chunks = std::max<long long>(max_chunks, (long long)er_gemm_plane_floats(p.rows, p.k) / 4);
+    }
+    const int blocks = (int)std::min<long long>((max_chunks + 255) / 256, 2LL * er::kSmCount);
+    er::launch_pdl(split_planes_kernel, dim3(blocks, cnt), dim3(256), 0, st, jobs);
+    ++launches;
+  }
+  er::count_launches(launches);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_gemm_planes(const float* A, int64_t lda, int32_t a_mn_major, const float* b_hi, const float* b_lo,
+                              const float* bias, float* C, int64_t ldc, int64_t M, int64_t N, int64_t K,
+                              const er_bn_stats_t* bn, void* ws, size_t ws_bytes, er_stream_t stream) {
+  if (bn && bias) return er::fail(ER_ERR_INVALID_ARG, "er_gemm_planes: with bn the bias goes in bn->bias");
+  if (bn && er::ceil_div(N, er::gemm::BN) > 256) return er::fail(ER_ERR_INVALID_ARG, "er_gemm_planes: N too large");
+  return gemm_impl(A, lda, a_mn_major, nullptr, 0, 0, b_hi, b_lo, bias, C, ldc, M, N, K, bn, ws, ws_bytes, stream);
 }

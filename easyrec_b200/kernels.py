@@ -599,8 +599,9 @@ def gemm_ready(t):
 _gemm_ws = {}
 
 
-def gemm(a, b, bias=None, out=None):
-  """out[M,N] = a[M,K] @ b[K,N] (+ bias) on the tensor cores (3xTF32).  a / b may be transposed views."""
+def gemm(a, b, bias=None, out=None, planes=None):
+  """out[M,N] = a[M,K] @ b[K,N] (+ bias) on the tensor cores (3xTF32).  a / b may be transposed views.
+  planes: b's pre-split (hi, lo) planes (DensePlanes.view), read instead of b; the result is bit-identical."""
   lib = _lib.load()
   M, Ka = a.shape
   Kb, N = b.shape
@@ -610,7 +611,8 @@ def gemm(a, b, bias=None, out=None):
     # read through their strides (transposed views in place); a 128x128 tensor-core tile would be all padding
     return gemm_small(a, b, bias, out)
   a, lda, a_unit = _gemm_operand(a, 'a')      # a_unit == 1: k contiguous -> K-major
-  b, ldb, b_unit = _gemm_operand(b, 'b')      # b_unit == 1: n contiguous -> MN-major
+  if planes is None:
+    b, ldb, b_unit = _gemm_operand(b, 'b')    # b_unit == 1: n contiguous -> MN-major
   if out is None:
     out = torch.empty(M, N, dtype=torch.float32, device=a.device)
   assert out.stride(1) == 1
@@ -622,6 +624,11 @@ def gemm(a, b, bias=None, out=None):
     if ws is None or ws.numel() < nbytes:
       ws = torch.empty(nbytes, dtype=torch.uint8, device=a.device)
       _gemm_ws[key] = ws
+  if planes is not None:
+    _lib.check(lib.er_gemm_planes(_p(a), lda, 0 if a_unit else 1, _p(planes[0]), _p(planes[1]), _p(bias), _p(out),
+                                  out.stride(0), M, N, Ka, None, _p(ws), 0 if ws is None else ws.numel(), _stream()),
+               'er_gemm_planes')
+    return out
   _lib.check(lib.er_gemm(_p(a), lda, 0 if a_unit else 1, _p(b), ldb, 1 if b_unit else 0, _p(bias), _p(out),
                          out.stride(0), M, N, Ka, _p(ws), 0 if ws is None else ws.numel(), _stream()), 'er_gemm')
   return out
@@ -656,9 +663,10 @@ def gemm_small(a, b, bias=None, out=None):
 _gemm_bn_ws = {}
 
 
-def gemm_bn(a, b, bias, moving_mean, moving_var, eps, momentum):
+def gemm_bn(a, b, bias, moving_mean, moving_var, eps, momentum, planes=None):
   """z = a @ b on the tensor cores, with the batch-norm statistics of z + bias from the GEMM epilogue.
-  Returns (z, save_mean, save_rstd), or None when the problem would be split along K (caller falls back)."""
+  Returns (z, save_mean, save_rstd), or None when the problem would be split along K (caller falls back).
+  planes: b's pre-split (hi, lo) planes (DensePlanes.view), read instead of b; the result is bit-identical."""
   lib = _lib.load()
   M, Ka = a.shape
   Kb, N = b.shape
@@ -666,7 +674,8 @@ def gemm_bn(a, b, bias, moving_mean, moving_var, eps, momentum):
   if N < 8 or Ka < 8 or M < 8 or lib.er_gemm_workspace_bytes(M, N, Ka) != 0:
     return None
   a, lda, a_unit = _gemm_operand(a, 'a')
-  b, ldb, b_unit = _gemm_operand(b, 'b')
+  if planes is None:
+    b, ldb, b_unit = _gemm_operand(b, 'b')
   z = torch.empty(M, N, dtype=torch.float32, device=a.device)
   mean = torch.empty(N, dtype=torch.float32, device=a.device)
   rstd = torch.empty(N, dtype=torch.float32, device=a.device)
@@ -677,9 +686,49 @@ def gemm_bn(a, b, bias, moving_mean, moving_var, eps, momentum):
     ws = torch.zeros(nbytes, dtype=torch.uint8, device=a.device)   # counters must start at zero
     _gemm_bn_ws[key] = ws
   bn = _lib.ErBnStats(_p(bias), _p(mean), _p(rstd), _p(moving_mean), _p(moving_var), eps, momentum)
+  if planes is not None:
+    _lib.check(lib.er_gemm_planes(_p(a), lda, 0 if a_unit else 1, _p(planes[0]), _p(planes[1]), None, _p(z),
+                                  z.stride(0), M, N, Ka, ctypes.byref(bn), _p(ws), ws.numel(), _stream()),
+               'er_gemm_planes')
+    return z, mean, rstd
   _lib.check(lib.er_gemm_bn(_p(a), lda, 0 if a_unit else 1, _p(b), ldb, 1 if b_unit else 0, _p(z), z.stride(0),
                             M, N, Ka, ctypes.byref(bn), _p(ws), ws.numel(), _stream()), 'er_gemm_bn')
   return z, mean, rstd
+
+
+class DensePlanes(object):
+  """Pre-split tf32 hi / lo planes of dense-layer kernels W[in, out], in the layout er_gemm_planes reads: per kernel
+  the planes of W^T (rows = out, k = in: the forward's B) and of W (rows = in, k = out: dX's B), in one buffer.
+  refresh() re-splits every kernel from its current values in one launch; it reads the tensors' storage, so a
+  kernel must stay the same storage (a view that is written in place) for as long as its planes are used."""
+
+  def __init__(self, kernels, device):
+    lib = _lib.load()
+    self.kernels = list(kernels)
+    for w in self.kernels:
+      assert w.dim() == 2 and w.dtype == torch.float32 and w.is_cuda and w.is_contiguous()
+    jobs = []
+    for w in self.kernels:
+      n_in, n_out = w.shape
+      jobs.append((n_out, n_in, 1, n_out))   # W^T: rows out, k in
+      jobs.append((n_in, n_out, n_out, 1))   # W: rows in, k out
+    sizes = [int(lib.er_gemm_plane_floats(rows, k)) for rows, k, _, _ in jobs]
+    self.buf = torch.empty(2 * sum(sizes), dtype=torch.float32, device=device)
+    self.planes = []
+    self.jobs = (_lib.ErGemmPlane * len(jobs))()
+    off = 0
+    for i, ((rows, k, ld_row, ld_k), n) in enumerate(zip(jobs, sizes)):
+      hi, lo = self.buf[off:off + n], self.buf[off + n:off + 2 * n]
+      off += 2 * n
+      self.planes.append((hi, lo))
+      self.jobs[i] = _lib.ErGemmPlane(_p(self.kernels[i // 2]), ld_row, ld_k, rows, k, _p(hi), _p(lo))
+
+  def refresh(self):
+    _lib.check(_lib.load().er_gemm_split_planes(self.jobs, len(self.planes), _stream()), 'er_gemm_split_planes')
+
+  def view(self, i, transposed):
+    """(hi, lo) of kernel i: transposed=False for the forward (B = W), True for dX (B = W^T)."""
+    return self.planes[2 * i + (1 if transposed else 0)]
 
 
 def bn_act_apply(z, bias, gamma, beta, mean, rstd, relu, y=None):

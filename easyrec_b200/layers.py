@@ -22,6 +22,7 @@ BN_MOMENTUM = 0.99
 _OVERLAP_DW_DX = os.environ.get('ER_OVERLAP_DW_DX', '1') == '1'
 _side = {}
 _defer = {'on': False, 'dirty': set()}
+_planes = {'on': None}
 
 
 class defer_dw_join(object):
@@ -44,6 +45,42 @@ class defer_dw_join(object):
     return False
 
 
+def tower_kernels(model):
+  """Kernels of the model's dense layers whose forward and dX run on the tensor-core GEMM (both sides at least 8): the
+  ones whose tf32 planes a trainer splits once per step (kernels.DensePlanes)."""
+  return [m.kernel for m in model.modules()
+          if isinstance(m, DenseLayer) and m.kernel.requires_grad and min(m.kernel.shape) >= 8]
+
+
+class use_planes(object):
+  """Inside this context a dense layer whose kernel is in `planes` (a kernels.DensePlanes refreshed from the
+  kernels' current values, which must not change inside the context) gives its forward and dX GEMMs the
+  pre-split planes instead of the kernel; the products are bit-identical.  The trainer wraps the forward and
+  backward pass of each step in it, right after the refresh; any other run splits the kernel in the GEMM."""
+
+  def __init__(self, planes):
+    self.planes = planes
+    self.index = {id(w): i for i, w in enumerate(planes.kernels)} if planes is not None else {}
+
+  def __enter__(self):
+    self.prev = _planes['on']
+    _planes['on'] = self
+    return self
+
+  def __exit__(self, *exc):
+    _planes['on'] = self.prev
+    return False
+
+
+def _kernel_planes(kernel):
+  """(forward planes, dX planes) of kernel while a use_planes context covers it, else (None, None)."""
+  ctx = _planes['on']
+  i = ctx.index.get(id(kernel)) if ctx is not None else None
+  if i is None:
+    return None, None
+  return ctx.planes.view(i, False), ctx.planes.view(i, True)
+
+
 def _side_stream(device):
   s = _side.get(device)
   if s is None:
@@ -60,15 +97,17 @@ class _DenseBNAct(torch.autograd.Function):
     ctx.kernel_param = kernel
     if hasattr(kernel, '_er_uses'):
       kernel._er_uses += 1
+    fwd_planes, ctx.dx_planes = _kernel_planes(kernel)
+    pk = {} if fwd_planes is None else {'planes': fwd_planes}
     fused = None
     if gamma is not None and training:
       # batch statistics come out of the GEMM epilogue; one elementwise pass normalises + activates
-      fused = K.gemm_bn(x, kernel, bias, moving_mean, moving_var, BN_EPS, BN_MOMENTUM)
+      fused = K.gemm_bn(x, kernel, bias, moving_mean, moving_var, BN_EPS, BN_MOMENTUM, **pk)
     if fused is not None:
       z, mean, rstd = fused
       y = K.bn_act_apply(z, bias, gamma, beta, mean, rstd, relu)
     else:
-      z = K.gemm(x, kernel)
+      z = K.gemm(x, kernel, **pk)
       y, mean, rstd = K.bias_bn_act_fwd(z, bias, gamma, beta, moving_mean, moving_var, BN_EPS,
                                         BN_MOMENTUM, training, relu, ws)
     ctx.relu = relu
@@ -90,6 +129,7 @@ class _DenseBNAct(torch.autograd.Function):
       gk = dst.view_as(dst)
     else:
       gk = torch.empty(x.shape[1], gz.shape[1], dtype=torch.float32, device=x.device)
+    pk = {} if ctx.dx_planes is None else {'planes': ctx.dx_planes}
     if ctx.needs_input_grad[0] and x.is_cuda and _OVERLAP_DW_DX:
       # dW (split-K, few tiles) and dX (many tiles) are independent: fork dW onto a side stream so the two
       # fill the 132 SMs together (captured as a fork/join inside the step's CUDA graph).  Outputs are
@@ -99,7 +139,7 @@ class _DenseBNAct(torch.autograd.Function):
       side.wait_stream(cur)
       with torch.cuda.stream(side):
         K.gemm(x.t(), gz, out=gk)
-      gx = K.gemm(gz, kernel.t())
+      gx = K.gemm(gz, kernel.t(), **pk)
       if _defer['on']:
         # joined by defer_dw_join.__exit__; the operands must outlive this function on the side stream
         gz.record_stream(side)
@@ -109,7 +149,7 @@ class _DenseBNAct(torch.autograd.Function):
         cur.wait_stream(side)
     else:
       K.gemm(x.t(), gz, out=gk)
-      gx = K.gemm(gz, kernel.t()) if ctx.needs_input_grad[0] else None
+      gx = K.gemm(gz, kernel.t(), **pk) if ctx.needs_input_grad[0] else None
     return gx, gk, gbias, ggamma, gbeta, None, None, None, None, None
 
 

@@ -186,6 +186,10 @@ class Trainer(object):
     self.dense_opt = FlatDenseOptimizer(named, dense_optimizer, lr, l2_of=l2, beta1=db1, beta2=db2,
                                         adagrad_init=adagrad_init)
     self.beta1, self.beta2 = beta1, beta2
+    # the tower kernels' tf32 planes, split at the head of every step's forward and backward (L.use_planes): they are
+    # then never stale, whatever wrote the weights between steps (optimizer, checkpoint restore, replica broadcast)
+    kernels = L.tower_kernels(model)
+    self.planes = K.DensePlanes(kernels, kernels[0].device) if kernels and kernels[0].is_cuda else None
     # dense_lr_fn: a second optimizer_config for everything that is not an embedding table (easy_rec_model.py:446-467):
     # its own schedule and beta powers in its own device block; otherwise one block serves both optimizers
     self.dense_lr_fn = dense_lr_fn
@@ -235,18 +239,21 @@ class Trainer(object):
   def _segment_compute(self, features, labels, next_features=None):
     """lookup -> model -> loss -> backward -> dense grads into the flat buffer."""
     self.dense_opt.zero_grad()
-    logits = self.model(features)
-    if next_features is not None:
-      # row-sharded tables: the id half of the NEXT batch's exchange reads no table, so it runs beside this step's
-      # backward and the next lookup only promotes it (InputLayer.prefetch_exchange)
-      self.input_layer.prefetch_exchange(next_features)
-    sw = features.get('sample_weight') if isinstance(features, dict) else None
-    if sw is not None:   # data_config.sample_weight (input/input.py:140-141 -> EasyRecModel._sample_weight)
-      loss, probs = self.model.loss(logits, labels, sample_weight=sw)
-    else:
-      loss, probs = self.model.loss(logits, labels)
-    with L.defer_dw_join():   # kernel-gradient GEMMs overlap the rest of the backward chain
-      loss.backward()
+    if self.planes is not None:
+      self.planes.refresh()
+    with L.use_planes(self.planes):
+      logits = self.model(features)
+      if next_features is not None:
+        # row-sharded tables: the id half of the NEXT batch's exchange reads no table, so it runs beside this step's
+        # backward and the next lookup only promotes it (InputLayer.prefetch_exchange)
+        self.input_layer.prefetch_exchange(next_features)
+      sw = features.get('sample_weight') if isinstance(features, dict) else None
+      if sw is not None:   # data_config.sample_weight (input/input.py:140-141 -> EasyRecModel._sample_weight)
+        loss, probs = self.model.loss(logits, labels, sample_weight=sw)
+      else:
+        loss, probs = self.model.loss(logits, labels)
+      with L.defer_dw_join():   # kernel-gradient GEMMs overlap the rest of the backward chain
+        loss.backward()
     self.dense_opt.gather_grads()
     self._step_pending = list(self.input_layer._pending)
     return loss.detach(), probs

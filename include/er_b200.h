@@ -513,6 +513,25 @@ size_t er_gemm_bn_workspace_bytes(int64_t M, int64_t N);
 int er_gemm_bn(const float* A, int64_t lda, int32_t a_mn_major, const float* B, int64_t ldb,
                int32_t b_mn_major, float* C, int64_t ldc, int64_t M, int64_t N, int64_t K,
                const er_bn_stats_t* bn, void* ws, size_t ws_bytes, er_stream_t stream);
+/* Pre-split B operands (the dense towers' weights, split once per step instead of once per 128-row output tile).
+ * er_gemm_split_planes writes, for each job, src(row, k) = src[row*ld_row + k*ld_k] (rows x k, any strides) as
+ * hi = tf32(x) and lo = x - hi planes of er_gemm_plane_floats(rows, k) floats each, in the K-major swizzled tile order
+ * er_gemm_planes reads, zero-padded to whole tiles; hi / lo 16-byte aligned.  One launch per 32 jobs.
+ * er_gemm_planes is er_gemm (bn NULL) or er_gemm_bn (bn given, bias NULL) with B given as the planes of its
+ * [N x K] K-major form (rows = N): forward of a dense layer W[in,out] -> the planes of W^T (ld_row 1, ld_k out),
+ * dX -> the planes of W (ld_row out, ld_k 1).  The products are bit-identical to er_gemm / er_gemm_bn on B. */
+typedef struct {
+  const float* src;
+  int64_t ld_row, ld_k;   /* in floats */
+  int64_t rows, k;
+  float* hi;
+  float* lo;
+} er_gemm_plane_t;
+size_t er_gemm_plane_floats(int64_t rows, int64_t K);
+int er_gemm_split_planes(const er_gemm_plane_t* planes, int32_t n, er_stream_t stream);
+int er_gemm_planes(const float* A, int64_t lda, int32_t a_mn_major, const float* b_hi, const float* b_lo,
+                   const float* bias, float* C, int64_t ldc, int64_t M, int64_t N, int64_t K,
+                   const er_bn_stats_t* bn, void* ws, size_t ws_bytes, er_stream_t stream);
 /* y = act((z + bias - mean) * rstd * gamma + beta) with given statistics (one elementwise pass). */
 int er_bn_act_apply(const float* z, const float* bias, const float* gamma, const float* beta,
                     const float* mean, const float* rstd, int64_t batch, int32_t units, int32_t relu,
