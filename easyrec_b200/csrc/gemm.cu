@@ -11,8 +11,9 @@
 //   - an operand whose K index is contiguous (activations in forward/dX, W[in,out] in dX) is stored with
 //     16 B vector stores, 8 threads per row;
 //   - an operand whose M/N index is contiguous (W[in,out] in forward, X and dY in dW) is transposed on its
-//     way into shared memory: a warp loads 16 k-rows x 8 contiguous M/N elements (full 32 B sectors) and
-//     scatters them with 4 B stores that fall in 32 different banks;
+//     way into shared memory: a thread loads a 4 (k) x 4 (M/N) block as four 16 B rows (a warp reads 4 k-rows
+//     x 128 contiguous bytes), transposes it in registers and stores 4 k of each M/N row with one 16 B store
+//     per plane, as the K-major path does;
 // so no transposed copy of any matrix is ever made.
 //
 // CTA = 128x128 output tile (one k-slice of it under split-K), 2 warpgroups:
@@ -196,20 +197,20 @@ __device__ __forceinline__ float4 mask_chunk(float4 v, int nvalid) {
   return v;
 }
 
-// Which 4 elements thread (warp, lane) moves in pass j (0..3) of a k-block, relative to the tile origin:
+// Which 4 elements thread (warp, lane) loads in pass j (0..3) of a k-block, relative to the tile origin:
 //   K-major : row r = lane/8 + 4*warp + 32*j (M/N), k = 4*(lane%8) .. +3
-//   MN-major: k = 16*(j%2) + lane%16, M/N = 8*(2*warp + j/2) + 4*(lane/16) .. +3
-// In both cases the load is only ISSUED (predicated, destination zeroed); elements past the K / MN edge are
-// cleared by mask_chunk when the registers are consumed.
+//   MN-major: the thread owns a 4 (k) x 4 (M/N) block and pass j loads its k row j:
+//             k = 4*kq + j, M/N = 4*mq .. +3,  kq = 4*(warp%2) + (lane/2)%4,  mq = 8*(warp/2) + 2*(lane/8) + lane%2
+// A warp's MN-major load reads 4 k rows x 128 contiguous bytes.  Rows past K or M/N are not loaded (predicated,
+// destination zeroed); the partial chunk at the K (K-major) or M/N (MN-major) edge is cleared by mask_chunk when
+// the registers are staged.
 struct Pos {
   int mn, k;   // first element's tile-relative M/N row and k column
 };
 __device__ __forceinline__ Pos pos_of(int mn_major, int warp, int lane, int j) {
   if (!mn_major) return Pos{(lane >> 3) + 4 * warp + 32 * j, 4 * (lane & 7)};
-  return Pos{8 * (2 * warp + (j >> 1)) + 4 * (lane >> 4), 16 * (j & 1) + (lane & 15)};
-}
-__device__ __forceinline__ int pos_nvalid(int mn_major, Pos p, int mn0, int mn_end, int k0, int k_end) {
-  return mn_major ? mn_end - (mn0 + p.mn) : k_end - (k0 + p.k);
+  const int kq = 4 * (warp & 1) + ((lane >> 1) & 3), mq = 8 * (warp >> 1) + 2 * (lane >> 3) + (lane & 1);
+  return Pos{4 * mq, 4 * kq + j};
 }
 __device__ __forceinline__ float4 load_pos(const float* __restrict__ P, long long ld, int mn_major, Pos p,
                                            int mn0, int mn_end, int k0, int k_end) {
@@ -226,24 +227,38 @@ __device__ __forceinline__ float4 load_pos(const float* __restrict__ P, long lon
 __device__ __forceinline__ uint32_t swz(int row, int k) {
   return (uint32_t)row * 128u + (uint32_t)((((k >> 2) ^ (row & 7)) << 4) + ((k & 3) << 2));
 }
-// hi / lo of one thread's 4 elements into the tile pair at `hi_tile` (lo tile kTileBytes further)
-__device__ __forceinline__ void store_pos(uint32_t hi_tile, int mn_major, Pos p, float4 v) {
+// hi / lo of 4 elements of tile row `row`, k = k4 .. k4+3, into the tile pair at `hi_tile` (lo tile kTileBytes
+// further)
+__device__ __forceinline__ void store_chunk(uint32_t hi_tile, int row, int k4, float4 v) {
   float4 hi, lo;
   split_tf32(v.x, hi.x, lo.x); split_tf32(v.y, hi.y, lo.y);
   split_tf32(v.z, hi.z, lo.z); split_tf32(v.w, hi.w, lo.w);
+  const uint32_t o = hi_tile + swz(row, k4);
+  asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
+  asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o + kTileBytes), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
+}
+// One thread's share of a k-block (the 4 passes `v`, loaded at `p`) into the tile pair at `hi_tile`.  Tile rows at
+// or past `rows` are never read by the tensor core and are not written.  An MN-major block is transposed in
+// registers, so each of its 4 M/N rows takes one 16 B store of 4 consecutive k per plane.  In a quarter-warp (8
+// lanes) those stores hit rows 4*mq + e with mq%2 = 0, 1 and k chunks kq = 4 consecutive values: under the 128 B
+// swizzle the 8 lanes land in 8 different 16 B chunk columns, i.e. in all 32 banks once (no conflict).
+__device__ __forceinline__ void store_block(uint32_t hi_tile, int mn_major, const Pos (&p)[4], const float4 (&v)[4],
+                                            int rows, int mn0, int mn_end, int k0, int k_end) {
   if (!mn_major) {
-    const uint32_t o = hi_tile + swz(p.mn, p.k);
-    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
-    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(o + kTileBytes), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w) : "memory");
-  } else {
-    const float h4[4] = {hi.x, hi.y, hi.z, hi.w}, l4[4] = {lo.x, lo.y, lo.z, lo.w};
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const uint32_t o = hi_tile + swz(p.mn + e, p.k);
-      asm volatile("st.shared.f32 [%0], %1;" ::"r"(o), "f"(h4[e]) : "memory");
-      asm volatile("st.shared.f32 [%0], %1;" ::"r"(o + kTileBytes), "f"(l4[e]) : "memory");
-    }
+    for (int j = 0; j < 4; ++j)
+      if (p[j].mn < rows) store_chunk(hi_tile, p[j].mn, p[j].k, mask_chunk(v[j], k_end - (k0 + p[j].k)));
+    return;
   }
+  if (p[0].mn >= rows) return;
+  const int nvalid = mn_end - (mn0 + p[0].mn);
+  float4 x[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) x[j] = mask_chunk(v[j], nvalid);
+  store_chunk(hi_tile, p[0].mn + 0, p[0].k, make_float4(x[0].x, x[1].x, x[2].x, x[3].x));
+  store_chunk(hi_tile, p[0].mn + 1, p[0].k, make_float4(x[0].y, x[1].y, x[2].y, x[3].y));
+  store_chunk(hi_tile, p[0].mn + 2, p[0].k, make_float4(x[0].z, x[1].z, x[2].z, x[3].z));
+  store_chunk(hi_tile, p[0].mn + 3, p[0].k, make_float4(x[0].w, x[1].w, x[2].w, x[3].w));
 }
 
 struct Welford {
@@ -299,12 +314,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tf32x3_kernel(Args a) {
   auto stage_out = [&](int kb, const float4 (&xa)[4], const float4 (&xb)[4]) {
     const int k0 = k_begin + kb * BK;
     const uint32_t st = smem_base + (uint32_t)(kb % kStages) * kStageBytes;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      store_pos(st, a.a_mn, pa[j], mask_chunk(xa[j], pos_nvalid(a.a_mn, pa[j], m0, a.M, k0, k_end)));
-      if (!kPreB && pb[j].mn < NM)
-        store_pos(st + 2 * kTileBytes, a.b_mn, pb[j], mask_chunk(xb[j], pos_nvalid(a.b_mn, pb[j], n0, a.N, k0, k_end)));
-    }
+    store_block(st, a.a_mn, pa, xa, BM, m0, a.M, k0, k_end);
+    if constexpr (!kPreB) store_block(st + 2 * kTileBytes, a.b_mn, pb, xb, NM, n0, a.N, k0, k_end);
   };
   // pre-split B: k-block kb's two planes -> stage kb % kStages (thread 0; the stage's previous wgmma's have retired)
   auto issue_b = [&](int kb) {

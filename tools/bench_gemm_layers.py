@@ -1,8 +1,9 @@
-"""Time the critical-path dense-tower GEMMs of the C2 DeepFM step one shape at a time: the forward (er_gemm_bn,
-batch statistics in the epilogue, as a DNN layer with batch norm runs it in training) and dX = dY.W^T (er_gemm) of
-the six tower layers at batch 8192.  Each row gives the kernel time from CUDA events over --iters launches replayed
-from a CUDA graph; the same GEMM reading the pre-split weight planes (kernels.DensePlanes) is timed beside it and its
-outputs are checked to be bit-identical.  Prints one JSON line per shape and the card it ran on."""
+"""Time the dense-tower GEMMs of the C2 DeepFM step one shape at a time: the forward (er_gemm_bn, batch statistics in
+the epilogue, as a DNN layer with batch norm runs it in training), dX = dY.W^T and dW = X^T.dY (er_gemm) of the six
+tower layers at batch 8192.  Each row gives the time per call from CUDA events over --iters calls replayed from a CUDA
+graph; for dW (split along K = batch) that is everything the call enqueues, the split-K reduction included.  The
+forward and dX GEMMs reading the pre-split weight planes (kernels.DensePlanes) are timed beside them and their outputs
+are checked to be bit-identical.  Prints one JSON line per shape and the card it ran on."""
 import argparse
 import json
 import os
@@ -62,7 +63,7 @@ def main():
   g = torch.Generator(device=dev).manual_seed(7)
   presplit = hasattr(K, 'DensePlanes')
   print(json.dumps({'card': card(), 'presplit_available': presplit}))
-  tot = {'current': 0.0, 'presplit': 0.0}
+  tot = {'current': 0.0, 'presplit': 0.0, 'dW': 0.0}
   for kin, kout in LAYERS:
     pitch = (kin + 3) // 4 * 4
     x = torch.randn(B, pitch, device=dev, generator=g)[:, :kin]
@@ -95,7 +96,14 @@ def main():
                                                      r1 if isinstance(r1, tuple) else (r1,)))
         row['bit_identical'] = same and torch.equal(mm0, mm) and torch.equal(mv0, mv)
       print(json.dumps(row))
-  print(json.dumps({'total_current_us': tot['current'], 'total_presplit_us': tot['presplit'] if presplit else None}))
+    # dW as DenseLayer's backward runs it: X^T (a transposed view of the pitched activations) times dY
+    gk = torch.empty(kin, kout, device=dev)
+    row = {'gemm': 'dW', 'M': kin, 'K': B, 'N': kout,
+           'current_us': timeit(lambda: K.gemm(x.t(), gz, out=gk), args.iters)}
+    tot['dW'] += row['current_us']
+    print(json.dumps(row))
+  print(json.dumps({'total_current_us': tot['current'], 'total_presplit_us': tot['presplit'] if presplit else None,
+                    'total_dW_us': tot['dW']}))
 
 
 if __name__ == '__main__':
