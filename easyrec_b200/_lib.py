@@ -97,6 +97,8 @@ SIGNATURES = {
     'er_fingerprint64_host': (ctypes.c_uint64, [ctypes.c_char_p, c_sz]),
     'er_csv_parse': (c_i32, [c_vp, c_sz, ctypes.c_char, ctypes.POINTER(ErCsvCol), c_i32, c_i64, c_i32,
                              ctypes.POINTER(c_i64), ctypes.POINTER(c_sz)]),
+    'er_csv_parse_lines': (c_i32, [c_vp, c_sz, ctypes.c_char, ctypes.POINTER(ErCsvCol), c_i32, c_i64, c_i32, c_i64, c_i64,
+                                   ctypes.POINTER(c_i64), ctypes.POINTER(c_sz), ctypes.POINTER(c_i64)]),
     'er_fingerprint64_i64': (c_i32, [c_vp, c_i64, c_vp]),
     'er_load_embed': (c_i32, [ctypes.c_char_p, ctypes.c_char_p, c_i32, c_i32, c_i32, c_i64, c_vp, c_vp]),
     'er_embedding_fwd': (c_i32, [

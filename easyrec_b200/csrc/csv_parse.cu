@@ -152,11 +152,17 @@ extern "C" int er_fingerprint64_i64(const int64_t* values, int64_t n, uint64_t* 
   return ER_OK;
 }
 
-extern "C" int er_csv_parse(const char* buf, size_t len, char sep, er_csv_col_t* cols, int32_t n_cols,
-                            int64_t max_rows, int32_t n_threads, int64_t* n_rows, size_t* consumed) {
+// er_csv_parse_lines: line j of the buffer (0-based) is parsed when j >= line_phase and (j - line_phase) is a
+// multiple of line_stride -- rank r of N reads lines r::N of a file this way (dataset.shard(N, r), input/input.py:
+// 1018-1023).  Every newline is scanned, only the kept lines are split into fields.  Stops after max_rows kept lines;
+// *lines_seen = complete lines passed over (kept or not) up to *consumed, so the caller carries the file's line index.
+extern "C" int er_csv_parse_lines(const char* buf, size_t len, char sep, er_csv_col_t* cols, int32_t n_cols,
+                                  int64_t max_rows, int32_t n_threads, int64_t line_stride, int64_t line_phase,
+                                  int64_t* n_rows, size_t* consumed, int64_t* lines_seen) {
   using namespace er;
-  ER_REQUIRE(buf && cols && n_rows && consumed, "null argument");
+  ER_REQUIRE(buf && cols && n_rows && consumed && lines_seen, "null argument");
   ER_REQUIRE(n_cols > 0 && max_rows >= 0, "bad n_cols / max_rows");
+  ER_REQUIRE(line_stride >= 1 && line_phase >= 0 && line_phase < line_stride, "bad line_stride / line_phase");
   for (int c = 0; c < n_cols; ++c) {
     const er_csv_col_t& k = cols[c];
     ER_REQUIRE(k.kind >= ER_CSV_SKIP && k.kind <= ER_CSV_HASH_STEP_LIST, "unknown column kind");
@@ -167,20 +173,27 @@ extern "C" int er_csv_parse(const char* buf, size_t len, char sep, er_csv_col_t*
     ER_REQUIRE(k.kind != ER_CSV_F32_VEC || k.width > 0, "vector column needs width");
     cols[c].n_vals = 0;
   }
-  // ---- complete lines in the buffer (the tail without '\n' is left to the caller) ----
-  std::vector<size_t> starts;
-  starts.reserve((size_t)std::min<int64_t>(max_rows, 1 << 20) + 1);
+  // ---- the kept complete lines of the buffer: [starts[r], ends[r]) with ends[r] at the '\n' (the tail without '\n' is
+  // left to the caller) ----
+  std::vector<size_t> starts, ends;
+  starts.reserve((size_t)std::min<int64_t>(max_rows, 1 << 20));
+  ends.reserve(starts.capacity());
   size_t pos = 0;
+  int64_t seen = 0;
   while ((int64_t)starts.size() < max_rows && pos < len) {
     const char* nl = (const char*)std::memchr(buf + pos, '\n', len - pos);
     if (!nl) break;
-    starts.push_back(pos);
+    if (seen >= line_phase && (seen - line_phase) % line_stride == 0) {
+      starts.push_back(pos);
+      ends.push_back((size_t)(nl - buf));
+    }
+    ++seen;
     pos = (size_t)(nl - buf) + 1;
   }
   const int64_t rows = (int64_t)starts.size();
-  starts.push_back(pos);
   *n_rows = rows;
   *consumed = pos;
+  *lines_seen = seen;
   if (rows == 0) return ER_OK;
   const int T = (int)std::max<int64_t>(1, std::min<int64_t>(n_threads > 0 ? n_threads : 1, (rows + 255) / 256));
   std::vector<LineErr> errs(T);
@@ -194,7 +207,7 @@ extern "C" int er_csv_parse(const char* buf, size_t len, char sep, er_csv_col_t*
         std::vector<Span> f((size_t)n_cols);
         for (int64_t r = r0; r < r1 && errs[t].row < 0; ++r) {
           const char* p = buf + starts[r];
-          const char* e = buf + starts[r + 1] - 1;          // the '\n'
+          const char* e = buf + ends[r];                    // the '\n'
           if (e > p && e[-1] == '\r') --e;
           int c = 0;
           while (c < n_cols) {
@@ -220,7 +233,7 @@ extern "C" int er_csv_parse(const char* buf, size_t len, char sep, er_csv_col_t*
   };
   auto report = [&](int t) {
     const er_csv_col_t& k = cols[errs[t].col];
-    return fail(ER_ERR_INVALID_ARG, "er_csv_parse: line " + std::to_string(errs[t].row + 1) + ", field " +
+    return fail(ER_ERR_INVALID_ARG, "er_csv_parse: line " + std::to_string(line_phase + errs[t].row * line_stride + 1) + ", field " +
                                         std::to_string(errs[t].col + 1) + " is not a valid " +
                                         (k.kind == ER_CSV_F32 || k.kind == ER_CSV_F32_VEC || k.kind == ER_CSV_F32_LIST ? "float"
                                          : is_kv(k.kind)                                  ? "key:weight list"
@@ -421,4 +434,11 @@ extern "C" int er_csv_parse(const char* buf, size_t len, char sep, er_csv_col_t*
   });
   if (bad >= 0) return report(bad);
   return ER_OK;
+}
+
+// every line of the buffer: the stride-1 case of er_csv_parse_lines
+extern "C" int er_csv_parse(const char* buf, size_t len, char sep, er_csv_col_t* cols, int32_t n_cols,
+                            int64_t max_rows, int32_t n_threads, int64_t* n_rows, size_t* consumed) {
+  int64_t seen = 0;
+  return er_csv_parse_lines(buf, len, sep, cols, n_cols, max_rows, n_threads, 1, 0, n_rows, consumed, &seen);
 }

@@ -102,6 +102,9 @@ class EasyRecEstimator(object):
         and world_size > 1
     if rank is None:
       rank = int(os.environ.get('RANK', 0)) if world_size > 1 else 0
+    self._rank, self._world = int(rank), int(world_size)
+    self._group = None        # gloo group of the end-of-data agreement and the metric reduction (made on first use)
+    self.agree_seconds, self.agree_calls = 0.0, 0
     self.input_layer, self.model, self._opt = builder.build_model(
         pipeline_config, self._batch_size, device, generator=gen,
         cpu_generator=torch.Generator().manual_seed(seed), default_seq_len=default_seq_len, world=world_size, rank=rank,
@@ -128,6 +131,46 @@ class EasyRecEstimator(object):
     return self._ep
 
   @property
+  def rank(self):
+    return self._rank
+
+  @property
+  def world_size(self):
+    return self._world
+
+  def _host_group(self):
+    """one gloo group over all ranks, for the small host collectives of train / evaluate / predict"""
+    if self._group is None:
+      import torch.distributed as dist
+      self._group = dist.new_group(backend='gloo')
+    return self._group
+
+  def _agree(self, flags, op):
+    """element-wise MIN or MAX of this rank's flags over all ranks: one int32 all-reduce on the host"""
+    import torch.distributed as dist
+    t0 = time.perf_counter()
+    t = torch.tensor([int(bool(f)) for f in flags], dtype=torch.int32)
+    dist.all_reduce(t, op=dist.ReduceOp.MIN if op == 'min' else dist.ReduceOp.MAX, group=self._host_group())
+    self.agree_seconds += time.perf_counter() - t0
+    self.agree_calls += 1
+    return [bool(x) for x in t.tolist()]
+
+  def _passes(self, input_fn, ahead, want_more, again):
+    """this rank's batches over the passes train() makes: (features, labels, next batch of the same pass or None); a
+    new pass over input_fn() starts when one ends while again(passes made) holds, unless the pass was empty."""
+    epoch = 0
+    while True:
+      feeder = readers.DeviceFeeder(readers.Prefetcher(input_fn(), depth=2), self._device, depth=2, lookahead=ahead)
+      self.last_feeder = feeder
+      n = 0
+      for item in _with_next(feeder, ahead, want_more):
+        n += 1
+        yield item
+      epoch += 1
+      if n == 0 or not again(epoch):
+        return
+
+  @property
   def feature_configs(self):
     return config_util.get_feature_configs(self._pipeline_config)
 
@@ -150,7 +193,12 @@ class EasyRecEstimator(object):
     thread (readers.Prefetcher).  fetch_loss_every_step: read the loss of EVERY step back to the host (what a per-step
     logging hook costs; bench.py's end-to-end number) - through pinned slots, one step behind the device
     (_LossReader), so the host prepares step k + 1 while step k runs; `last_loss_value` is the newest value read and,
-    when train() returns, the last step's."""
+    when train() returns, the last step's.
+
+    world_size > 1: before each step the ranks agree (one host all-reduce over a gloo group) on whether every rank holds
+    this step's batch and, with row-sharded tables, the next one; the run stops at the first step some rank cannot
+    make, and the next batch's id exchange is prefetched only when every rank has one, so no rank enters a collective
+    another rank skips."""
     limit = steps if steps is not None else (max_steps or self.train_config.num_steps or None)
     every = max(int(self.train_config.log_step_count_steps), 1)
     t0, n0 = time.time(), self.global_step
@@ -158,18 +206,25 @@ class EasyRecEstimator(object):
     # data_config.num_epochs: 0 = pass over the data again and again until the step limit (input/input.py:1033-1040
     # dataset.repeat); without a step limit one pass is made
     epochs = int(self._pipeline_config.data_config.num_epochs)
-    done = False
-    epoch = 0
     reader = _LossReader(self._device) if fetch_loss_every_step else None
-    while not done:
-      seen = self.global_step
-      # row-sharded tables: train_step is told the NEXT batch, whose id exchange then runs beside the current step
-      ahead = 1 if self._ep else 0
-      feeder = readers.DeviceFeeder(readers.Prefetcher(input_fn(), depth=2), self._device, depth=2, lookahead=ahead)
-      self.last_feeder = feeder
-      for feats, labels, nxt in _with_next(feeder, ahead, lambda: limit is None or self.global_step - n0 + 1 < limit):
+    # row-sharded tables: train_step is told the NEXT batch, whose id exchange then runs beside the current step
+    ahead = 1 if self._ep else 0
+    stream = self._passes(input_fn, ahead, lambda: limit is None or self.global_step - n0 + 1 < limit,
+                          lambda epoch: limit is not None and not (epochs > 0 and epoch >= epochs))
+    try:
+      while True:
+        item = next(stream, None)   # (a rank whose pass ended has started the next one, when there is one)
+        nxt = None if item is None else item[2]
+        if self._world > 1:
+          have, have_next = self._agree([item is not None, nxt is not None or not ahead], 'min')
+          if not have:
+            break
+          if not have_next:
+            nxt = None
+        elif item is None:
+          break
         # host parsing and the H2D copies run ahead of the device step
-        loss, _ = self.trainer.train_step(feats, labels, next_features=None if nxt is None else nxt[0])
+        loss, _ = self.trainer.train_step(item[0], item[1], next_features=None if nxt is None else nxt[0])
         self.global_step += 1
         if reader is not None:
           self.last_loss_value = reader.push(loss)
@@ -178,11 +233,9 @@ class EasyRecEstimator(object):
           logging.info('global_step = %d, loss = %.6f, global_step/sec = %.2f', self.global_step, float(loss),
                        (self.global_step - n0) / max(dt, 1e-9))
         if limit is not None and self.global_step - n0 >= limit:
-          done = True
           break
-      epoch += 1
-      if limit is None or self.global_step == seen or (epochs > 0 and epoch >= epochs):
-        done = True
+    finally:
+      stream.close()
     if reader is not None and loss is not None:
       self.last_loss_value = reader.flush()      # the last step's loss: every step's result has reached the host
       return self.last_loss_value
@@ -215,13 +268,45 @@ class EasyRecEstimator(object):
         out.append((which, self.input_layer.sparse_names.index(feat), conf.reduction))
     return out
 
+  def _eval_batches(self, input_fn, steps=None):
+    """(host features, device features, device labels, own) for evaluate / predict: this rank's batches (at most
+    `steps`).  Row-sharded tables with world_size > 1: every forward takes part in the exchange, so a rank whose batches
+    are used up repeats a forward of its last batch (own = False: outputs dropped) until every rank is out - one host
+    all-reduce per forward decides."""
+    gang = self._ep and self._world > 1
+    it = iter(input_fn())
+    n, had, last = 0, False, None
+    while True:
+      item = next(it, None) if (steps is None or n < steps) else None
+      if gang:
+        anyone, stranded = self._agree([item is not None, item is None and not had], 'max')
+        if not anyone:
+          return
+        if stranded:
+          raise ValueError('evaluate / predict under row-sharded tables: a rank has no full batch of its own to take '
+                           'part in the exchanges of the others')
+      elif item is None:
+        return
+      if item is None:
+        yield None, last[0], last[1], False
+        continue
+      had = True
+      n += 1
+      last = readers.to_device(item[0], item[1], self._device)
+      yield item[0], last[0], last[1], True
+
   def evaluate(self, input_fn, steps=None, hooks=None, checkpoint_path=None, name=None):
     """One pass over input_fn() (or `steps` batches) -> {metric name: value, 'global_step'} for eval_config.metrics_set
     (no metrics_set: auc).  The streaming metrics (auc at AUC.num_thresholds thresholds as tf.metrics.auc computes it,
     max_f1, the mean / root-mean errors; every task tower of a multi-task model under '<metric>_<tower_name>') are
     accumulated on the device, batch by batch (metrics.MetricSet over er_auc_hist); the grouped AUCs gauc / session_auc
     are computed on the host over the collected predictions, as the reference's py_func does (core/metrics.py:59-106).
-    `auc_exact` is the exact ROC AUC of the single binary head (what the thresholded `auc` approximates)."""
+    `auc_exact` is the exact ROC AUC of the single binary head (what the thresholded `auc` approximates).
+
+    world_size > 1: each rank evaluates what its input_fn yields, then the metrics are reduced over all ranks - the
+    threshold histograms summed, the error totals and counts summed in rank order, `auc_exact` / `gauc` /
+    `session_auc` computed over the labels, probabilities and keys of all ranks in rank order - so every rank returns
+    the same dict, that of one process evaluating the union of the batches."""
     heads = metrics.heads_of(self.model)
     mset = metrics.MetricSet(self.eval_config.metrics_set, heads, self._device)
     single = len(heads) == 1 and heads[0][0] == '' and heads[0][1] == 'CLASSIFICATION'
@@ -230,33 +315,49 @@ class EasyRecEstimator(object):
     keys_all = [[] for _ in groups]
     B = self.input_layer.batch_size
     n = 0
-    for feats, labels in input_fn():
-      for k, (_, pos, _) in enumerate(groups):
-        keys_all[k].append(feats['sparse_fea'][pos * B:(pos + 1) * B].cpu().numpy())
-      feats, labels = readers.to_device(feats, labels, self._device)
+    for host, feats, labels, own in self._eval_batches(input_fn, steps):
       logits = self._forward_eval(feats)
+      if not own:
+        continue
+      for k, (_, pos, _) in enumerate(groups):
+        keys_all[k].append(host['sparse_fea'][pos * B:(pos + 1) * B].cpu().numpy())
       if heads:
         mset.update(logits, labels)
       if single:
         probs_all.append(torch.sigmoid(logits))
         labels_all.append(labels)
       n += 1
-      if steps is not None and n >= steps:
-        break
+    lab = prob = None
+    if probs_all:
+      lab, prob = torch.cat(labels_all).cpu().numpy(), torch.cat(probs_all).cpu().numpy()
+    keys = [np.concatenate(k) if k else None for k in keys_all]
+    if self._world > 1:
+      import torch.distributed as dist
+      group = self._host_group()
+      mset.all_reduce(group)
+      parts = [None] * self._world
+      dist.all_gather_object(parts, (n, lab, prob, keys), group=group)
+      n = sum(p[0] for p in parts)
+      got = [p for p in parts if p[1] is not None]
+      if got:
+        lab, prob = np.concatenate([p[1] for p in got]), np.concatenate([p[2] for p in got])
+        keys = [np.concatenate([p[3][k] for p in got]) for k in range(len(groups))]
     out = {'global_step': self.global_step}
     if n and heads:
       out.update(mset.result())
-    if probs_all:
-      lab, prob = torch.cat(labels_all).cpu().numpy(), torch.cat(probs_all).cpu().numpy()
+    if lab is not None:
       out['auc_exact'] = metrics.auc(lab, prob)
-      for (which, _, reduction), keys in zip(groups, keys_all):
-        out[which] = float(metrics.gauc(lab, prob, np.concatenate(keys), reduction))
+      for (which, _, reduction), k in zip(groups, keys):
+        out[which] = float(metrics.gauc(lab, prob, k, reduction))
     return out
 
   def predict(self, input_fn, predict_keys=None, hooks=None, checkpoint_path=None, yield_single_examples=True):
-    for feats, labels in input_fn():
-      feats, _ = readers.to_device(feats, labels, self._device)
+    """{'logits', 'probs'} per batch of input_fn(); world_size > 1: this rank's batches (every rank has to iterate to the
+    end under row-sharded tables, whose forwards exchange rows)."""
+    for _, feats, _, own in self._eval_batches(input_fn):
       logits = self._forward_eval(feats)
+      if not own:
+        continue
       yield {'logits': logits.cpu().numpy(), 'probs': torch.sigmoid(logits).cpu().numpy()}
 
   def save(self, model_dir=None, embedding_parts=False):
@@ -310,14 +411,15 @@ class EasyRecEstimator(object):
 
 
 def train_and_evaluate(pipeline_config_path, train_input_fn=None, eval_input_fn=None, device='cuda:0', **kw):
-  """main._train_and_evaluate_impl (main.py:296-400) for the supported model families."""
+  """main._train_and_evaluate_impl (main.py:296-400) for the supported model families.  With world_size > 1 every rank
+  reads its own shard of train_input_path and eval_input_path (readers.make_input with this rank and world size)."""
   est = EasyRecEstimator(pipeline_config_path, device=device, **kw)
   cfg = est._pipeline_config
   if train_input_fn is None:
     path = cfg.train_input_path
-    train_input_fn = lambda: readers.make_input(cfg, est.input_layer, path)  # noqa: E731
+    train_input_fn = lambda: readers.make_input(cfg, est.input_layer, path, est.rank, est.world_size)  # noqa: E731
   est.train(train_input_fn)
   if eval_input_fn is None and cfg.eval_input_path:
     epath = cfg.eval_input_path
-    eval_input_fn = lambda: readers.make_input(cfg, est.input_layer, epath)  # noqa: E731
+    eval_input_fn = lambda: readers.make_input(cfg, est.input_layer, epath, est.rank, est.world_size)  # noqa: E731
   return est, (est.evaluate(eval_input_fn) if eval_input_fn else {})

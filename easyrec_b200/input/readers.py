@@ -10,6 +10,7 @@ parser: Fingerprint64(bytes) % hash_bucket_size (StringToHashBucketFast, feature
 fields go to the device untouched and are hashed there from their decimal text (input/input.py:541-543).
 """
 import ctypes
+import glob
 import os
 
 import numpy as np
@@ -211,15 +212,25 @@ class DummyInput(object):
 class CSVInput(object):
   """CSVInput (input/csv_input.py): delimiter-separated text, one sample per line, columns in
   data_config.input_fields order; labels from label_fields.  Only Id / Raw / Sequence / Tag features.
-  The file bytes go through the library's native parser (er_csv_parse) straight into the batch arrays."""
+  The file bytes go through the library's native parser (er_csv_parse_lines) straight into the batch arrays.
 
-  def __init__(self, pipeline_config, input_layer, path, batch_size=None, seq_sep='|', engine='native', n_threads=None):
+  task_index / task_num: worker `task_index` of `task_num` reads the lines `task_index::task_num` of the file (after the
+  header), record by record like the reference's dataset.shard(task_num, task_index) (input/input.py:1018-1023); its
+  batches are cut from its own lines in file order.  The parser threads default to the single-process rule divided by
+  LOCAL_WORLD_SIZE, so the workers of one host share its cores."""
+
+  def __init__(self, pipeline_config, input_layer, path, batch_size=None, seq_sep='|', engine='native', n_threads=None,
+               task_index=0, task_num=1):
     self.cfg = pipeline_config
     self.il = input_layer
     self.path = path
     assert engine in ('native', 'python')
     self.engine = engine
-    self.n_threads = n_threads or max(1, min(16, (os.cpu_count() or 1) // 2))
+    if not 0 <= task_index < task_num:
+      raise ValueError('task_index %d is not in [0, task_num %d)' % (task_index, task_num))
+    self.task_index, self.task_num = int(task_index), int(task_num)
+    local_world = max(1, int(os.environ.get('LOCAL_WORLD_SIZE', 1)))
+    self.n_threads = n_threads or max(1, min(16, (os.cpu_count() or 1) // 2) // local_world)
     dc = pipeline_config.data_config
     self.sep = dc.separator or ','
     self.fields = [f.input_name for f in dc.input_fields]
@@ -353,8 +364,9 @@ class CSVInput(object):
     return plan
 
   def _parse(self, data, size, plan, list_cap, n_batches=1):
-    """one er_csv_parse call on `size` bytes at `data` (address or bytes) for up to n_batches * batch_size lines
-    -> (n_rows, consumed, {field: arrays}), or None when a list column needs a larger array."""
+    """one er_csv_parse_lines call on `size` bytes at `data` (address or bytes) for up to n_batches * batch_size of this
+    worker's lines - the first line of the buffer and every task_num-th one after it -> (n_rows, consumed, lines passed
+    over, {field: arrays}), or None when a list column needs a larger array."""
     B = self.batch_size * n_batches
     list_cap = list_cap * n_batches
     cols = (_lib.ErCsvCol * len(self.fields))()
@@ -393,18 +405,19 @@ class CSVInput(object):
           c.kv_sep = default.encode()     # the plan's default slot carries the key / weight separator
       if kind != _lib.CSV_SKIP:
         c.out = out[name][0].ctypes.data
-    n_rows, consumed = ctypes.c_int64(0), ctypes.c_size_t(0)
-    st = _lib.load().er_csv_parse(data, size, self.sep.encode(), cols, len(self.fields), B, self.n_threads,
-                                  ctypes.byref(n_rows), ctypes.byref(consumed))
+    n_rows, consumed, seen = ctypes.c_int64(0), ctypes.c_size_t(0), ctypes.c_int64(0)
+    st = _lib.load().er_csv_parse_lines(data, size, self.sep.encode(), cols, len(self.fields), B, self.n_threads,
+                                        self.task_num, 0, ctypes.byref(n_rows), ctypes.byref(consumed),
+                                        ctypes.byref(seen))
     if st == _lib.ER_ERR_WORKSPACE:
       return None
-    _lib.check(st, 'er_csv_parse')
+    _lib.check(st, 'er_csv_parse_lines')
     for i, name in enumerate(self.fields):
       if cols[i].kind in _STEP_KINDS:
         out[name] = (out[name][0][:cols[i].n_vals], out[name][1], out[name][2])
       elif cols[i].kind in _LIST_KINDS:
         out[name] = (out[name][0][:cols[i].n_vals], out[name][1]) + tuple(w[:cols[i].n_vals] for w in out[name][2:])
-    return n_rows.value, consumed.value, out
+    return n_rows.value, consumed.value, seen.value, out
 
   @staticmethod
   def _slice_chunk(cols, plan, k, B):
@@ -429,9 +442,19 @@ class CSVInput(object):
   def _batches_native(self):
     """the file is memory-mapped and parsed in place; one er_csv_parse call takes a CHUNK of several batches (about
     32K lines) so that the parser's threads are started once per chunk, not once per batch, and have enough lines each;
-    the last, short chunk of the file is parsed batch by batch."""
+    the last, short chunk of the file is parsed batch by batch.  `line` is the index (after the header) of the file line
+    at `off`; before each call `off` moves on to this worker's next line, (task_index - line) mod task_num lines on."""
     import mmap
     B = self.batch_size
+    N, me = self.task_num, self.task_index
+    line = 0
+
+    def own_line(off, line):
+      for _ in range((me - line) % N):     # (at most task_num - 1 other workers' lines)
+        nl = mm.find(b'\n', off)
+        off = nl + 1 if nl >= 0 else size  # (an unterminated last line of another worker: nothing left)
+        line += 1
+      return off, line
     plan = self._column_plan()
     list_cap = 16 * B
     chunk = max(1, 32768 // B)
@@ -444,30 +467,34 @@ class CSVInput(object):
         if self.cfg.data_config.with_header:      # the first line names the columns (csv_input.py:139-145)
           off = mm.find(b'\n') + 1 or size
         while chunk > 1:
+          off, line = own_line(off, line)
           res = self._parse(base + off, size - off, plan, list_cap, n_batches=chunk)
           if res is None:          # a list column outgrew its array
             list_cap *= 4
             continue
-          n_rows, consumed, cols = res
+          n_rows, consumed, seen, cols = res
           if n_rows < chunk * B:   # the end of the file is inside this chunk: batch by batch from here
             break
           off += consumed
+          line += seen
           for k in range(chunk):
             yield self._pack_columns(self._slice_chunk(cols, plan, k, B))
         while True:
+          off, line = own_line(off, line)
           res = self._parse(base + off, size - off, plan, list_cap)
           if res is None:          # a list column outgrew its array
             list_cap *= 4
             continue
-          n_rows, consumed, cols = res
+          n_rows, consumed, seen, cols = res
           if n_rows < B:           # end of file; a last line without '\n' still counts
             tail = bytes(mm[off:])
             if tail and not tail.endswith(b'\n'):
               res = self._parse(tail + b'\n', len(tail) + 1, plan, max(list_cap, len(tail)))
               if res is not None and res[0] == B:
-                yield self._pack_columns(res[2])
+                yield self._pack_columns(res[3])
             return                 # a ragged last batch does not fit the static plan: skipped
           off += consumed
+          line += seen
           yield self._pack_columns(cols)
       finally:
         del view
@@ -544,7 +571,9 @@ class CSVInput(object):
     with open(self.path, 'rb') as f:
       if self.cfg.data_config.with_header:
         f.readline()
-      for line in f:
+      for i, line in enumerate(f):
+        if i % self.task_num != self.task_index:   # another worker's line
+          continue
         buf.append(line.rstrip(b'\r\n').decode('utf-8', errors='surrogateescape').split(self.sep))
         if len(buf) == B:
           yield self._pack(buf)
@@ -648,14 +677,23 @@ class ParquetInput(object):
   cells belong to a TagFeature), Tag / Sequence features keep the whole list; a list-valued dense cell
   holds raw_input_dim values (the reference reads x[0] of a list cell, load_parquet.py:108-114, i.e. dim 1).  Like the
   reference's packed path the ids go to the device untouched and are bucketed there (`vals % num_buckets`,
-  parquet_input.py:221, or the feature's hash rule)."""
+  parquet_input.py:221, or the feature's hash rule).
 
-  def __init__(self, pipeline_config, input_layer, path, batch_size=None):
+  `path`: a list of files, or a string of comma-separated patterns, each expanded (sorted) in turn.  Worker task_index
+  of task_num reads file j of that list when j % task_num == task_index (parquet_input.py:36-57)."""
+
+  def __init__(self, pipeline_config, input_layer, path, batch_size=None, task_index=0, task_num=1):
     import pyarrow.parquet as pq   # optional dependency of this reader only
     self._pq = pq
     self.cfg = pipeline_config
     self.il = input_layer
-    self.paths = [path] if isinstance(path, str) else list(path)
+    if not 0 <= task_index < task_num:
+      raise ValueError('task_index %d is not in [0, task_num %d)' % (task_index, task_num))
+    self.all_paths = expand_paths(path)
+    self.paths = self.all_paths[task_index::task_num]
+    if not self.paths:
+      raise ValueError('ParquetInput: %d file(s) for task_num %d workers leave worker %d without a file; write at least '
+                       'task_num files' % (len(self.all_paths), task_num, task_index))
     self.labels = list(pipeline_config.data_config.label_fields)
     dc = pipeline_config.data_config
     self.weight_field = dc.sample_weight if dc.HasField('sample_weight') else None
@@ -845,8 +883,20 @@ def from_reference_packed(input_layer, fea_dict, sparse_fea_names):
   return feats
 
 
-def make_input(pipeline_config, input_layer, path):
-  """reader for data_config.input_type (CSVInput / ParquetInput / DummyInput)."""
+def expand_paths(path):
+  """a list of files as given, or a string of comma-separated patterns: each pattern expanded and sorted in turn (a
+  name without wildcards is kept as it is)."""
+  if not isinstance(path, str):
+    return list(path)
+  out = []
+  for p in path.strip().split(','):
+    out.extend(sorted(glob.glob(p)) if glob.has_magic(p) else [p])
+  return out
+
+
+def make_input(pipeline_config, input_layer, path, task_index=0, task_num=1):
+  """reader for data_config.input_type (CSVInput / ParquetInput / DummyInput); worker task_index of task_num reads its
+  shard of `path` (DummyInput: every worker its own constant batches, as before)."""
   from easyrec_b200 import builder
   dc = pipeline_config.data_config
   if dc.WhichOneof('sampler') is not None:
@@ -855,10 +905,10 @@ def make_input(pipeline_config, input_layer, path):
     raise NotImplementedError('data_config.%s: negative samplers are outside the hot-path scope' % dc.WhichOneof('sampler'))
   kind = builder.input_type_name(pipeline_config)
   if kind.startswith('Parquet'):
-    return ParquetInput(pipeline_config, input_layer, path)
+    return ParquetInput(pipeline_config, input_layer, path, task_index=task_index, task_num=task_num)
   if kind == 'DummyInput':
     return DummyInput(input_layer, n_labels=max(1, len(dc.label_fields)))
-  return CSVInput(pipeline_config, input_layer, path)
+  return CSVInput(pipeline_config, input_layer, path, task_index=task_index, task_num=task_num)
 
 
 class Prefetcher(object):

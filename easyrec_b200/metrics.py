@@ -86,6 +86,13 @@ class ConfusionAtThresholds(object):
     from easyrec_b200 import kernels as K
     K.auc_hist(predictions.detach().to(torch.float32), labels.detach().to(torch.float32), self.thr, self.hist)
 
+  def all_reduce(self, group):
+    """sum the histograms of all ranks (uint64 counts: exact, in any order)"""
+    import torch.distributed as dist
+    h = self.hist.cpu()
+    dist.all_reduce(h, op=dist.ReduceOp.SUM, group=group)
+    self.hist.copy_(h)
+
   def counts(self):
     """(tp, fn, tn, fp) float32 [T] (TF keeps the accumulators in float32 variables)."""
     h = self.hist.cpu().numpy()
@@ -123,6 +130,17 @@ class StreamingMean(object):
   def update(self, values):
     self.total += values.detach().double().sum()
     self.count += values.numel()
+
+  def all_reduce(self, group):
+    """totals and counts of all ranks, summed in rank order: every rank gets the same bits"""
+    import torch.distributed as dist
+    parts = [None] * dist.get_world_size(group)
+    dist.all_gather_object(parts, (float(self.total), self.count), group=group)
+    total = 0.0
+    for t, _ in parts:
+      total += t
+    self.total.fill_(total)
+    self.count = sum(c for _, c in parts)
 
   def result(self):
     return float(self.total) / max(self.count, 1)
@@ -174,6 +192,11 @@ class MetricSet(object):
         pred = lg if loss_type == 'L2_LOSS' else torch.sigmoid(lg)
         d = lab.to(torch.float32) - pred
         a.update(d.abs() if which == 'mean_absolute_error' else d * d)
+
+  def all_reduce(self, group):
+    """every accumulator reduced over the ranks of `group` (torch.distributed, host tensors)"""
+    for _, _, _, a in self.acc:
+      a.all_reduce(group)
 
   def result(self):
     out = {}

@@ -671,6 +671,13 @@ typedef struct {
 } er_csv_col_t;
 int er_csv_parse(const char* buf, size_t len, char sep, er_csv_col_t* cols, int32_t n_cols,
                  int64_t max_rows, int32_t n_threads, int64_t* n_rows, size_t* consumed);
+/* The same parse over every line_stride-th line of the buffer, from line line_phase on (0 <= line_phase <
+ * line_stride): the rows are the kept lines only, in buffer order; every newline is scanned but only kept lines are
+ * split into fields.  *lines_seen = complete lines passed over up to *consumed (kept or not).  Rank r of N reading
+ * lines r::N of a file passes line_stride = N and the phase of its next line.  er_csv_parse is line_stride 1. */
+int er_csv_parse_lines(const char* buf, size_t len, char sep, er_csv_col_t* cols, int32_t n_cols,
+                       int64_t max_rows, int32_t n_threads, int64_t line_stride, int64_t line_phase,
+                       int64_t* n_rows, size_t* consumed, int64_t* lines_seen);
 
 /* Fingerprint64 of the decimal text of each int64 (tf.as_string + the string hash): what an integer input of a
  * crossed / hashed column contributes (input/input.py:356-376).  HOST pointers. */
