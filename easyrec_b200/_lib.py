@@ -36,6 +36,7 @@ OPT_SGD, OPT_ADAGRAD, OPT_LAZY_ADAM, OPT_ADAM_ROWS, OPT_MOMENTUM = 0, 1, 2, 3, 4
 ACT_GELU, ACT_LEAKY_RELU, ACT_ELU, ACT_SELU, ACT_TANH, ACT_SWISH, ACT_SIGMOID = 1, 2, 3, 4, 5, 6, 7
 MAX_BUFS = 8
 ABI_VERSION = 3
+CRITEO_N_DENSE, CRITEO_N_CAT = 13, 26   # ER_CRITEO_N_DENSE / ER_CRITEO_N_CAT: values per sample of a binary part
 HYPER_LR, HYPER_BETA1_POWER, HYPER_BETA2_POWER, HYPER_GRAD_SCALE, HYPER_N = 0, 1, 2, 3, 4
 
 
@@ -100,6 +101,7 @@ SIGNATURES = {
     'er_csv_parse_lines': (c_i32, [c_vp, c_sz, ctypes.c_char, ctypes.POINTER(ErCsvCol), c_i32, c_i64, c_i32, c_i64, c_i64,
                                    ctypes.POINTER(c_i64), ctypes.POINTER(c_sz), ctypes.POINTER(c_i64)]),
     'er_fingerprint64_i64': (c_i32, [c_vp, c_i64, c_vp]),
+    'er_binary_unpack': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'er_load_embed': (c_i32, [ctypes.c_char_p, ctypes.c_char_p, c_i32, c_i32, c_i32, c_i64, c_vp, c_vp]),
     'er_embedding_fwd': (c_i32, [
         c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp,

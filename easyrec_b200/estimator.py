@@ -320,7 +320,7 @@ class EasyRecEstimator(object):
       if not own:
         continue
       for k, (_, pos, _) in enumerate(groups):
-        keys_all[k].append(host['sparse_fea'][pos * B:(pos + 1) * B].cpu().numpy())
+        keys_all[k].append(readers.host_ids(host, pos, B))
       if heads:
         mset.update(logits, labels)
       if single:
@@ -410,16 +410,25 @@ class EasyRecEstimator(object):
     return self
 
 
+def _input_path(cfg, which):
+  """what make_input reads for `which` ('train' / 'eval'): the BinaryDataInput of binary_<which>_input when the
+  <which>_path oneof holds it, else <which>_input_path"""
+  if cfg.WhichOneof(which + '_path') == 'binary_%s_input' % which:
+    return getattr(cfg, 'binary_%s_input' % which)
+  return getattr(cfg, which + '_input_path')
+
+
 def train_and_evaluate(pipeline_config_path, train_input_fn=None, eval_input_fn=None, device='cuda:0', **kw):
   """main._train_and_evaluate_impl (main.py:296-400) for the supported model families.  With world_size > 1 every rank
-  reads its own shard of train_input_path and eval_input_path (readers.make_input with this rank and world size)."""
+  reads its own shard of train_input_path and eval_input_path, or of binary_train_input and binary_eval_input
+  (readers.make_input with this rank and world size)."""
   est = EasyRecEstimator(pipeline_config_path, device=device, **kw)
   cfg = est._pipeline_config
   if train_input_fn is None:
-    path = cfg.train_input_path
+    path = _input_path(cfg, 'train')
     train_input_fn = lambda: readers.make_input(cfg, est.input_layer, path, est.rank, est.world_size)  # noqa: E731
   est.train(train_input_fn)
-  if eval_input_fn is None and cfg.eval_input_path:
-    epath = cfg.eval_input_path
+  epath = _input_path(cfg, 'eval')
+  if eval_input_fn is None and epath:
     eval_input_fn = lambda: readers.make_input(cfg, est.input_layer, epath, est.rank, est.world_size)  # noqa: E731
   return est, (est.evaluate(eval_input_fn) if eval_input_fn else {})

@@ -12,6 +12,7 @@ fields go to the device untouched and are hashed there from their decimal text (
 import ctypes
 import glob
 import os
+import re
 
 import numpy as np
 import torch
@@ -842,6 +843,201 @@ class ParquetInput(object):
     return self.batches()
 
 
+_CRITEO_COLUMN = re.compile(r'([fc])([1-9][0-9]*)$')
+
+
+def criteo_columns(pipeline_config, input_layer):
+  """The column maps of a CriteoInput plan -> (slot_cols, raw_cols): the category column of every id slot in
+  input_layer.sparse_names order, the dense column of every raw column of dense_fea.  Inputs map by name
+  (input/criteo_input.py:76-86): fK is dense column K-1, cK category column K-1, `label` the label.  Only what the files
+  can feed without host work is accepted: IdFeatures over cK with hash_bucket_size / num_buckets (bucketed on the
+  device like any integer id) and RawFeatures of raw_input_dim 1 over fK; every other use raises naming the feature."""
+  from easyrec_b200 import builder
+  dc = pipeline_config.data_config
+  if list(dc.label_fields) != ['label']:
+    raise ValueError('CriteoInput: label_fields must be ["label"], the files\' one label (got %s)' % list(dc.label_fields))
+  if dc.HasField('sample_weight'):
+    raise NotImplementedError('CriteoInput: sample_weight %r has no source in the binary files' % dc.sample_weight)
+  types = builder.input_field_types(pipeline_config)
+  col = {}
+  for fc in config_util.get_feature_configs(pipeline_config):
+    name = fc.feature_name if fc.HasField('feature_name') else fc.input_names[0]
+    ftype = builder.ftype_name(fc)
+    if ftype not in ('IdFeature', 'RawFeature'):
+      raise NotImplementedError('feature %s: a %s needs host work or a source the CriteoInput files do not have; '
+                                'only IdFeature and RawFeature are read from them' % (name, ftype))
+    src = fc.input_names[0]
+    m = _CRITEO_COLUMN.match(src)
+    k = int(m.group(2)) if m else 0
+    if len(fc.input_names) != 1 or not m or k > (_lib.CRITEO_N_DENSE if m.group(1) == 'f' else _lib.CRITEO_N_CAT):
+      raise ValueError('feature %s: input %r is not one of the CriteoInput columns f1..f13 / c1..c26'
+                       % (name, ', '.join(fc.input_names)))
+    if ftype == 'RawFeature':
+      if m.group(1) != 'f':
+        raise ValueError('feature %s: a RawFeature reads a dense column f1..f13, not %r' % (name, src))
+      if builder.raw_boundaries(fc) is not None:
+        raise NotImplementedError('feature %s: a bucketized RawFeature (boundaries) is bucketed on the host; CriteoInput '
+                                  'batches are unpacked on the device' % name)
+      if fc.raw_input_dim != 1:
+        raise ValueError('feature %s: a CriteoInput dense column holds one value, raw_input_dim is %d'
+                         % (name, fc.raw_input_dim))
+    else:
+      if m.group(1) != 'c':
+        raise ValueError('feature %s: an IdFeature reads a category column c1..c26, not %r' % (name, src))
+      if fc.hash_bucket_size <= 0 and fc.num_buckets <= 0:
+        raise NotImplementedError('feature %s: a CriteoInput id needs hash_bucket_size or num_buckets' % name)
+      if types.get(src) == 'STRING':
+        raise NotImplementedError('feature %s: input field %r is declared STRING, whose ids are hashed from their text on '
+                                  'the host; the CriteoInput categories are integers' % (name, src))
+    col[name] = k - 1
+  slot_cols = [col[n] for n in input_layer.sparse_names]
+  raw_cols = [0] * input_layer.n_dense
+  for n in input_layer.raw_names:
+    raw_cols[input_layer.raw_cols[n][0]] = col[n]
+  return np.array(slot_cols, np.int32), np.array(raw_cols, np.int32)
+
+
+class BinaryBatch(object):
+  """One CriteoInput batch as the files hold it: label int32 [B], dense fp32 [B, 13] and cat int32 [B, 26] (the uint32
+  bits, read as the reference's declared tf.int32), with the column maps of the reader's plan.  It becomes the batch of
+  the other readers - sparse_fea int64 [n_slot * B] feature-major, dense_fea fp32 [B, n_raw], labels fp32 [B] - on the
+  device, by er_binary_unpack (DeviceFeeder on its copy stream, to_device)."""
+
+  def __init__(self, label, dense, cat, slot_cols, raw_cols, maps=None):
+    self.label, self.dense, self.cat = label, dense, cat
+    self.slot_cols, self.raw_cols = slot_cols, raw_cols
+    self._maps = {} if maps is None else maps   # device -> the maps there; shared by the batches of one reader
+
+  @property
+  def batch_size(self):
+    return self.label.numel()
+
+  def ids(self, pos):
+    """host int64 ids of id slot `pos` (what sparse_fea[pos * B:(pos + 1) * B] holds after the unpack)"""
+    return self.cat[:, int(self.slot_cols[pos])].numpy().astype(np.int64)
+
+  def unpack(self, label, dense, cat, out=(None, None, None)):
+    """er_binary_unpack on the current stream over the batch's arrays where they are now (on the device, or the host
+    tensors under the kernel doubles) -> (features, labels) in the form of the other readers."""
+    from easyrec_b200 import kernels as K
+    dev = str(label.device)
+    if dev not in self._maps:
+      self._maps[dev] = K.binary_maps(self.slot_cols, self.raw_cols, label.device)
+    sparse, dense_fea, labels = K.binary_unpack(label, dense, cat, *self._maps[dev], *out)
+    feats = {}
+    if self.slot_cols.size:
+      feats['sparse_fea'] = sparse
+    if self.raw_cols.size:
+      feats['dense_fea'] = dense_fea
+    return feats, labels
+
+
+def host_ids(feats, pos, batch_size):
+  """host int64 ids of id slot `pos` of a host batch (a reader's dict or a BinaryBatch)"""
+  if isinstance(feats, BinaryBatch):
+    return feats.ids(pos)
+  return feats['sparse_fea'][pos * batch_size:(pos + 1) * batch_size].cpu().numpy()
+
+
+def criteo_parts(binary_paths):
+  """BinaryDataInput -> [(label, dense, category) file paths]: entry i of each list expanded with glob and sorted, per
+  kind, then appended in list order (input/criteo_input.py:37-52); the three lists must match file for file."""
+  n = (len(binary_paths.label_path), len(binary_paths.dense_path), len(binary_paths.category_path))
+  if len(set(n)) != 1:
+    raise ValueError('CriteoInput: label_path (%d), dense_path (%d) and category_path (%d) must have as many entries' % n)
+  parts = []
+  for lp, dp, cp in zip(binary_paths.label_path, binary_paths.dense_path, binary_paths.category_path):
+    got = [sorted(glob.glob(p)) for p in (lp, dp, cp)]
+    if len(set(len(g) for g in got)) != 1:
+      raise ValueError('CriteoInput: label_path %r, dense_path %r and category_path %r match %d, %d and %d files'
+                       % ((lp, dp, cp) + tuple(len(g) for g in got)))
+    parts.extend(zip(*got))
+  return parts
+
+
+def criteo_shard(total, task_index, task_num):
+  """(first sample, sample count) of worker task_index of task_num over `total` samples in file order: every worker
+  gets ceil(total / task_num) samples in one contiguous range, and the workers at or beyond total % task_num start one
+  sample early - so neighbouring ranges overlap and every worker has as many samples
+  (criteo_binary_reader.py:61-74)."""
+  avg, res = divmod(int(total), int(task_num))
+  if res == 0:
+    return avg * task_index, avg
+  return ((avg + 1) * task_index if task_index < res else avg * task_index + res - 1), avg + 1
+
+
+class CriteoBinaryInput(object):
+  """CriteoInput (input/criteo_input.py + input/criteo_binary_reader.py): per part three flat files - label int32,
+  dense 13 x float32 and category 26 x uint32 per sample.  Nothing is parsed: a batch is three byte ranges, read with
+  pread straight into its arrays, and yielded as a BinaryBatch that the device unpacks into the readers' batch form.
+
+  binary_paths: the BinaryDataInput of binary_train_input / binary_eval_input.  Worker task_index of task_num reads
+  the samples criteo_shard gives it, of the parts concatenated in order; batches are the next batch_size samples in
+  file order, across file boundaries, and the last partial batch is skipped (the plan's batch size is fixed)."""
+
+  def __init__(self, pipeline_config, input_layer, binary_paths, task_index=0, task_num=1, batch_size=None):
+    if isinstance(binary_paths, (str, bytes)) or not hasattr(binary_paths, 'label_path'):
+      raise ValueError('CriteoInput reads the binary parts named by binary_train_input / binary_eval_input '
+                       '(BinaryDataInput), not %r' % (binary_paths,))
+    if not 0 <= task_index < task_num:
+      raise ValueError('task_index %d is not in [0, task_num %d)' % (task_index, task_num))
+    self.slot_cols, self.raw_cols = criteo_columns(pipeline_config, input_layer)
+    self.batch_size = batch_size or input_layer.batch_size
+    self.parts = criteo_parts(binary_paths)
+    if not self.parts:
+      raise ValueError('CriteoInput: the binary paths match no file')
+    self.counts = []
+    for paths in self.parts:
+      n = os.path.getsize(paths[0]) // 4
+      for p, width in zip(paths, (4, 4 * _lib.CRITEO_N_DENSE, 4 * _lib.CRITEO_N_CAT)):
+        if os.path.getsize(p) != n * width:
+          raise ValueError('CriteoInput: %s holds %d bytes, %d samples of %d bytes expected' % (p, os.path.getsize(p), n, width))
+      self.counts.append(n)
+    self.starts = np.concatenate([[0], np.cumsum(self.counts, dtype=np.int64)])
+    self.start, self.n_samples = criteo_shard(int(self.starts[-1]), task_index, task_num)
+    self._maps = {}
+
+  def batches(self):
+    B = self.batch_size
+    fds = {}
+    try:
+      for k in range(self.n_samples // B):
+        yield self._read(self.start + k * B, B, fds), None
+    finally:
+      for fd in fds.values():
+        os.close(fd)
+
+  def _read(self, pos, n, fds):
+    """samples [pos, pos + n) of the concatenated parts, read into fresh arrays"""
+    label = np.empty(n, np.int32)
+    dense = np.empty((n, _lib.CRITEO_N_DENSE), np.float32)
+    cat = np.empty((n, _lib.CRITEO_N_CAT), np.int32)
+    arrs = [memoryview(a).cast('B') for a in (label, dense, cat)]
+    widths = (4, 4 * _lib.CRITEO_N_DENSE, 4 * _lib.CRITEO_N_CAT)
+    done = 0
+    f = int(np.searchsorted(self.starts, pos, side='right')) - 1
+    while done < n:
+      off = pos + done - int(self.starts[f])
+      take = min(n - done, self.counts[f] - off)
+      for kind, (p, w, buf) in enumerate(zip(self.parts[f], widths, arrs)):
+        fd = fds.get((f, kind))
+        if fd is None:
+          fd = fds[(f, kind)] = os.open(p, os.O_RDONLY)
+        dst, at = buf[done * w:(done + take) * w], off * w
+        while len(dst):
+          got = os.preadv(fd, [dst], at)
+          if got <= 0:
+            raise IOError('CriteoInput: %s ended before sample %d' % (p, off + take))
+          dst, at = dst[got:], at + got
+      done += take
+      f += 1
+    return BinaryBatch(torch.from_numpy(label), torch.from_numpy(dense), torch.from_numpy(cat), self.slot_cols,
+                       self.raw_cols, self._maps)
+
+  def __iter__(self):
+    return self.batches()
+
+
 def from_reference_packed(input_layer, fea_dict, sparse_fea_names):
   """The reference's packed feature dict (ParquetInput._to_fea_dict, input/parquet_input.py:201-239) -> the
   InputLayer's batch form.  fea_dict['sparse_fea'] = (vals int64 [L], lens int32 [n_feat * B]) with the lens
@@ -895,8 +1091,9 @@ def expand_paths(path):
 
 
 def make_input(pipeline_config, input_layer, path, task_index=0, task_num=1):
-  """reader for data_config.input_type (CSVInput / ParquetInput / DummyInput); worker task_index of task_num reads its
-  shard of `path` (DummyInput: every worker its own constant batches, as before)."""
+  """reader for data_config.input_type (CSVInput / ParquetInput / CriteoInput / DummyInput); worker task_index of
+  task_num reads its shard of `path` (DummyInput: every worker its own constant batches, as before).  CriteoInput takes
+  the BinaryDataInput message of binary_train_input / binary_eval_input as `path`."""
   from easyrec_b200 import builder
   dc = pipeline_config.data_config
   if dc.WhichOneof('sampler') is not None:
@@ -904,6 +1101,11 @@ def make_input(pipeline_config, input_layer, path, task_index=0, task_num=1):
     # input/sampler.py) are not something these readers produce
     raise NotImplementedError('data_config.%s: negative samplers are outside the hot-path scope' % dc.WhichOneof('sampler'))
   kind = builder.input_type_name(pipeline_config)
+  if kind == 'CriteoInput':
+    if isinstance(path, (str, bytes)):
+      raise ValueError('CriteoInput reads binary_train_input / binary_eval_input (BinaryDataInput: label_path, dense_path, '
+                       'category_path), not the string path %r' % (path,))
+    return CriteoBinaryInput(pipeline_config, input_layer, path, task_index=task_index, task_num=task_num)
   if kind.startswith('Parquet'):
     return ParquetInput(pipeline_config, input_layer, path, task_index=task_index, task_num=task_num)
   if kind == 'DummyInput':
@@ -1021,6 +1223,18 @@ class DeviceFeeder(object):
     with torch.cuda.stream(stream):
       if slot.consumed is not None:
         stream.wait_event(slot.consumed)
+      if isinstance(feats, BinaryBatch):
+        # the three arrays as read cross PCIe; er_binary_unpack makes the batch form in the slot's own device buffers
+        raw = [self._stage(slot, ('__binary', i), t, stream) for i, t in enumerate((feats.label, feats.dense, feats.cat))]
+        B, n_raw = feats.batch_size, feats.raw_cols.size
+        shapes = ((feats.slot_cols.size * B,), (B, n_raw), (B,))
+        if getattr(slot, 'unpacked', None) is None or [tuple(t.shape) for t in slot.unpacked] != list(shapes):
+          slot.unpacked = [torch.empty(sh, dtype=dt, device=self.device)
+                           for sh, dt in zip(shapes, (torch.int64, torch.float32, torch.float32))]
+        slot.batch = feats.unpack(*raw, out=slot.unpacked)
+        slot.ready = torch.cuda.Event()
+        slot.ready.record(stream)
+        return
       out = {}
       for k, v in feats.items():
         if isinstance(v, dict):
@@ -1036,7 +1250,7 @@ class DeviceFeeder(object):
   def __iter__(self):
     if not str(self.device).startswith('cuda'):
       for feats, labels in self.source:
-        yield feats, labels
+        yield feats.unpack(feats.label, feats.dense, feats.cat) if isinstance(feats, BinaryBatch) else (feats, labels)
       return
     import collections as _c
     stream = torch.cuda.Stream(device=self.device)
@@ -1070,6 +1284,8 @@ class DeviceFeeder(object):
 
 
 def to_device(feats, labels, device):
+  if isinstance(feats, BinaryBatch):
+    return feats.unpack(*(t.to(device, non_blocking=True) for t in (feats.label, feats.dense, feats.cat)))
   out = {}
   for k, v in feats.items():
     if isinstance(v, dict):

@@ -216,6 +216,46 @@ def auc_hist(probs, labels, thresholds, hist):
   return hist
 
 
+def binary_maps(slot_cols, raw_cols, device):
+  """the column maps of er_binary_unpack as device int32 tensors, each entry checked against its range on the host (the
+  kernel reads them from device memory unchecked)"""
+  out = []
+  for cols, hi, nm in ((slot_cols, _lib.CRITEO_N_CAT, 'slot_cols'), (raw_cols, _lib.CRITEO_N_DENSE, 'raw_cols')):
+    a = np.asarray(cols, np.int64).reshape(-1)
+    if a.size and (a.min() < 0 or a.max() >= hi):
+      raise _lib.ErError('%s entries must be in [0, %d)' % (nm, hi))
+    out.append(torch.from_numpy(a.astype(np.int32)).to(device))
+  if out[1].numel() > _lib.CRITEO_N_DENSE:
+    raise _lib.ErError('raw_cols has %d entries, at most %d' % (out[1].numel(), _lib.CRITEO_N_DENSE))
+  return tuple(out)
+
+
+def binary_unpack(label, dense, cat, slot_cols, raw_cols, sparse_fea=None, dense_fea=None, labels=None):
+  """er_binary_unpack: one CriteoInput batch (label int32 [B], dense fp32 [B, 13], cat int32 [B, 26] holding the uint32
+  bits) -> (sparse_fea int64 [n_slot * B] feature-major, dense_fea fp32 [B, n_raw], labels fp32 [B]).  slot_cols /
+  raw_cols: device int32 maps from binary_maps.  Outputs are written into the given tensors when passed."""
+  B = label.numel()
+  _chk(label, torch.int32, 'label')
+  _chk(dense, torch.float32, 'dense')
+  _chk(cat, torch.int32, 'cat')
+  _chk(slot_cols, torch.int32, 'slot_cols')
+  _chk(raw_cols, torch.int32, 'raw_cols')
+  if dense.numel() != B * _lib.CRITEO_N_DENSE or cat.numel() != B * _lib.CRITEO_N_CAT:
+    raise _lib.ErError('dense / cat must hold 13 / 26 values per label')
+  n_slot, n_raw = slot_cols.numel(), raw_cols.numel()
+  dev = label.device
+  sparse_fea = torch.empty(n_slot * B, dtype=torch.int64, device=dev) if sparse_fea is None else sparse_fea
+  dense_fea = torch.empty((B, n_raw), dtype=torch.float32, device=dev) if dense_fea is None else dense_fea
+  labels = torch.empty(B, dtype=torch.float32, device=dev) if labels is None else labels
+  _chk(sparse_fea, torch.int64, 'sparse_fea')
+  _chk(dense_fea, torch.float32, 'dense_fea')
+  _chk(labels, torch.float32, 'labels')
+  assert sparse_fea.numel() == n_slot * B and dense_fea.numel() == B * n_raw and labels.numel() == B
+  _lib.check(_lib.load().er_binary_unpack(_p(label), _p(dense), _p(cat), B, _p(slot_cols), n_slot, _p(raw_cols), n_raw,
+                                          _p(sparse_fea), _p(dense_fea), _p(labels), _stream()), 'er_binary_unpack')
+  return sparse_fea, dense_fea.view(B, n_raw), labels
+
+
 def shard_group_workspace(n_lookups, device):
   return torch.empty(_lib.load().er_shard_group_workspace_bytes(int(n_lookups)), dtype=torch.uint8, device=device)
 

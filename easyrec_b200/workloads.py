@@ -211,6 +211,28 @@ def write_c2_files(prefix, n_batches, batch_size, seed=20240, uniform=False):
   return prefix + '.tsv', prefix + '.parquet'
 
 
+def write_c2_binary(prefix, n_batches, batch_size, n_files, seed=20240, uniform=False):
+  """The C2 batches of `criteo_batch` as CriteoInput binary parts (input/criteo_binary_reader.py): n_files parts
+  `<prefix>_part<k>_{label,dense,category}.bin` of int32 labels, 13 float32 and 26 uint32 per sample, the samples split
+  evenly in order (the remainder in the last part).  The ids are taken mod 2^31, so that the reference's int32 reading
+  of the uint32 values keeps them.  Returns the (label, dense, category) glob patterns of a BinaryDataInput."""
+  ids, dense, labels = [], [], []
+  for i in range(n_batches):
+    x, d, l = criteo_batch(batch_size, seed + i, uniform=uniform)
+    ids.append(x.reshape(26, batch_size).T % 2**31)
+    dense.append(d)
+    labels.append(l)
+  ids, dense, labels = np.concatenate(ids), np.concatenate(dense), np.concatenate(labels)
+  n = labels.size
+  cuts = [k * (n // n_files) for k in range(n_files)] + [n]
+  for k in range(n_files):
+    lo, hi = cuts[k], cuts[k + 1]
+    labels[lo:hi].astype(np.int32).tofile('%s_part%03d_label.bin' % (prefix, k))
+    dense[lo:hi].astype(np.float32).tofile('%s_part%03d_dense.bin' % (prefix, k))
+    ids[lo:hi].astype(np.uint32).tofile('%s_part%03d_category.bin' % (prefix, k))
+  return tuple('%s_part*_%s.bin' % (prefix, kind) for kind in ('label', 'dense', 'category'))
+
+
 def c4_config_text(batch_size=4096, item_vocab=200_000_000, user_vocab=10_000_000, emb_dim=16, lr=0.01,
                    embedding_parallel=True):
   """C4 of BASELINE.json as a pipeline config: DSSM two towers (samples/model_config/dssm_on_taobao.config's shape:

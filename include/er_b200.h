@@ -683,6 +683,22 @@ int er_csv_parse_lines(const char* buf, size_t len, char sep, er_csv_col_t* cols
  * crossed / hashed column contributes (input/input.py:356-376).  HOST pointers. */
 int er_fingerprint64_i64(const int64_t* values, int64_t n, uint64_t* out);
 
+/* ---- CriteoInput batches (input/criteo_binary_reader.py, input/criteo_input.py:76-86) ----
+ * One batch of the binary parts, as read from the files: label int32[batch], dense float32[batch, 13] and cat
+ * uint32[batch, 26], row-major.  Writes the batch form of the other readers:
+ *   sparse_fea int64[n_slot * batch], feature-major: sparse_fea[s * batch + b] = (int64)(int32) cat[b, slot_cols[s]]
+ *     (the reference's declared tf.int32 output type);
+ *   dense_fea float32[batch, n_raw]: dense_fea[b, j] = dense[b, raw_cols[j]];
+ *   labels float32[batch] = (float) label.
+ * slot_cols int32[n_slot] (duplicates allowed) and raw_cols int32[n_raw] are DEVICE arrays whose entries the caller
+ * keeps in [0, 26) and [0, 13): they live in device memory, where this call cannot check them.  n_slot 0 / n_raw 0 skip
+ * that output (its pointers may then be null).  No allocation, no synchronisation. */
+#define ER_CRITEO_N_DENSE 13
+#define ER_CRITEO_N_CAT 26
+int er_binary_unpack(const int32_t* label, const float* dense, const uint32_t* cat, int64_t batch,
+                     const int32_t* slot_cols, int32_t n_slot, const int32_t* raw_cols, int32_t n_raw,
+                     int64_t* sparse_fea, float* dense_fea, float* labels, er_stream_t stream);
+
 /* ---- sharded-table restore: the LoadEmbed custom op (ops/src/load_dense_embed.cc:28-156;
  * python fallback compat/embedding_parallel_saver.py:141-173) ----
  * HOST function, HOST pointers (the op is a CPU kernel in the reference as well).  Reads every
