@@ -253,64 +253,86 @@ __device__ __forceinline__ void enqueue_long(const BwdArgs& a, int64_t start, in
 }
 
 // ---- one-row tables (ER_BUCKET_ONE_ROW slots): weighted column sums -----------------------------------------
-// CTA (slot f, chunk c) sums coef_b * g[b, cols of f] over its kOneRowChunk samples: lane groups take samples
+// Chunk c of slot f sums coef_b * g[b, cols of f] over its kOneRowChunk samples: lane groups take samples
 // g, g + G, ... in order, the groups are added in group order, the chunk partials in chunk order by the slot's
 // last CTA, which then applies the optimizer to the row: deterministic.  CTAs of other slots exit at once.
+// A slot gets or_chunks CTAs, sized on the average slot; CTA c takes chunks c, c + or_chunks, ... so a slot with
+// more segments than that is still covered.  Chunk c's partial sits at f + seg_begin / kOneRowChunk + c: slots are
+// disjoint and ordered by seg_begin, so the indices of different slots never meet (and stay below
+// max_one_row_parts).
 // Their shared memory is declared at namespace scope: the compiler then places it behind bk_fused_kernel's own
 // shared variables (s_warp at offset 0), the layout that kernel's code was measured with.
 __shared__ __align__(16) float s_or_part[1024];   // vec: G groups x LANES float4; scalar: 256 floats
 __shared__ int s_or_last;
+__shared__ long long s_or_row;
+
+// every live lookup of a one-row slot names the same row - K1 writes slot.row_offset for all of them, the row-sharded
+// exchange (sharded.ShardedLookup) the position of that one row in its send buffer - but any of them may be dropped
+// (-1): the row of the first live one, found block by block (all threads of the CTA call this), or -1
+__device__ __forceinline__ int64_t one_row_row(const BwdArgs& a, const er_slot_t& sl) {
+  for (int base = 0; base < sl.n_seg; base += blockDim.x) {
+    const int e = base + threadIdx.x;
+    const int64_t r = e < sl.n_seg ? a.or_rows[(int64_t)sl.seg_begin + e] : -1;
+    if (threadIdx.x == 0) s_or_row = -1;
+    __syncthreads();
+    if (r >= 0) s_or_row = r;
+    if (__syncthreads_or(r >= 0)) return s_or_row;
+  }
+  return -1;
+}
+
 template <int LANES>
 __device__ __forceinline__ void one_row_cta(const BwdArgs& a, int cta) {
-  const int f = cta / a.or_chunks, c = cta - f * a.or_chunks;
+  const int f = cta / a.or_chunks, c_first = cta - f * a.or_chunks;
   const er_slot_t sl = a.slots[f];
   if (sl.bucket_mode != ER_BUCKET_ONE_ROW) return;
   constexpr int L = LANES > 0 ? LANES : 1;
   constexpr int G = 256 / L;
   const int dim = a.dim;
-  const int s0 = c * bk::kOneRowChunk, s1 = min(sl.n_seg, s0 + bk::kOneRowChunk);
   const int used_chunks = (sl.n_seg + bk::kOneRowChunk - 1) / bk::kOneRowChunk;
-  if (s0 >= sl.n_seg) return;
+  if (c_first >= used_chunks) return;
+  const int used_ctas = min(a.or_chunks, used_chunks);
+  float* const parts = a.or_partials + ((int64_t)f + sl.seg_begin / bk::kOneRowChunk) * dim;   // [chunk][dim]
   const float* gbuf = a.gbufs.p[sl.out_buf];
-  // every lookup of a one-row slot resolves to the same row: K1 writes slot.row_offset for all of them, and the
-  // row-sharded exchange (sharded.ShardedLookup) the position of that one row in its send buffer
-  const int64_t row64 = a.or_rows[sl.seg_begin];
-  if (row64 < 0) return;
-  const uint32_t row = (uint32_t)row64;
   if constexpr (LANES > 0) {
     const int grp = threadIdx.x / LANES, lane = threadIdx.x % LANES;
-    float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
-    constexpr int U = 4;   // samples of a lane group in flight
-    for (int e = s0 + grp; e < s1; e += G * U) {
-      float4 v[U];
-      float coef[U];
-      bool use[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int ee = e + u * G;
-        use[u] = false;
-        if (ee < s1) {
-          const int64_t l = (int64_t)sl.seg_begin + ee;   // single-valued slot: lookup == segment
-          use[u] = a.or_rows[l] >= 0;                        // a dropped lookup contributes nothing
-          coef[u] = a.weights ? a.weights[l] : 1.0f;
-          if (a.seg_scale) coef[u] = __fmul_rn(coef[u], a.seg_scale[l]);
-          v[u] = reinterpret_cast<const float4*>(gbuf + (int64_t)ee * sl.out_stride + sl.out_col)[lane];
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u)
-        if (use[u]) f4_fma_sep(g, v[u], coef[u]);
-    }
-    reinterpret_cast<float4*>(s_or_part)[grp * LANES + lane] = g;
-    __syncthreads();
     float4 tot = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (threadIdx.x < LANES) {
-      for (int q = 0; q < G; ++q) f4_acc(tot, reinterpret_cast<float4*>(s_or_part)[q * LANES + threadIdx.x]);
-      __stcg(reinterpret_cast<float4*>(a.or_partials + ((int64_t)f * a.or_chunks + c) * dim) + threadIdx.x, tot);
+    for (int c = c_first; c < used_chunks; c += a.or_chunks) {
+      const int s0 = c * bk::kOneRowChunk, s1 = min(sl.n_seg, s0 + bk::kOneRowChunk);
+      float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+      constexpr int U = 4;   // samples of a lane group in flight
+      for (int e = s0 + grp; e < s1; e += G * U) {
+        float4 v[U];
+        float coef[U];
+        bool use[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int ee = e + u * G;
+          use[u] = false;
+          if (ee < s1) {
+            const int64_t l = (int64_t)sl.seg_begin + ee;   // single-valued slot: lookup == segment
+            use[u] = a.or_rows[l] >= 0;                        // a dropped lookup contributes nothing
+            coef[u] = a.weights ? a.weights[l] : 1.0f;
+            if (a.seg_scale) coef[u] = __fmul_rn(coef[u], a.seg_scale[l]);
+            v[u] = reinterpret_cast<const float4*>(gbuf + (int64_t)ee * sl.out_stride + sl.out_col)[lane];
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+          if (use[u]) f4_fma_sep(g, v[u], coef[u]);
+      }
+      reinterpret_cast<float4*>(s_or_part)[grp * LANES + lane] = g;
+      __syncthreads();
+      tot = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (threadIdx.x < LANES) {
+        for (int q = 0; q < G; ++q) f4_acc(tot, reinterpret_cast<float4*>(s_or_part)[q * LANES + threadIdx.x]);
+        __stcg(reinterpret_cast<float4*>(parts + (int64_t)c * dim) + threadIdx.x, tot);
+      }
+      __syncthreads();
     }
     __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) s_or_last = (atomicAdd(&a.or_tickets[f], 1) == used_chunks - 1);
+    if (threadIdx.x == 0) s_or_last = (atomicAdd(&a.or_tickets[f], 1) == used_ctas - 1);
     __syncthreads();
     if (s_or_last) {
       __threadfence();
@@ -319,7 +341,7 @@ __device__ __forceinline__ void one_row_cta(const BwdArgs& a, int cta) {
         const int q = base + grp;
         if (q < used_chunks)
           reinterpret_cast<float4*>(s_or_part)[grp * LANES + lane] =
-              __ldcg(reinterpret_cast<const float4*>(a.or_partials + ((int64_t)f * a.or_chunks + q) * dim) + lane);
+              __ldcg(reinterpret_cast<const float4*>(parts + (int64_t)q * dim) + lane);
         __syncthreads();
         if (threadIdx.x < LANES) {
           if (base == 0) tot = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -328,41 +350,47 @@ __device__ __forceinline__ void one_row_cta(const BwdArgs& a, int cta) {
         }
         __syncthreads();
       }
-      if (threadIdx.x < LANES) {
-        RowRegs r = load_row(a, row, threadIdx.x);
-        apply_row_vec(a, row, threadIdx.x, tot, 0, r);
-        if (threadIdx.x == 0) a.or_tickets[f] = 0;
+      const int64_t row = one_row_row(a, sl);
+      if (threadIdx.x < LANES && row >= 0) {
+        RowRegs r = load_row(a, (uint32_t)row, threadIdx.x);
+        apply_row_vec(a, (uint32_t)row, threadIdx.x, tot, 0, r);
       }
+      if (threadIdx.x == 0) a.or_tickets[f] = 0;
     }
   } else {
-    for (int col = 0; col < dim; ++col) {
-      float g = 0.f;
-      for (int e = s0 + threadIdx.x; e < s1; e += 256) {
-        const int64_t l = (int64_t)sl.seg_begin + e;
-        if (a.or_rows[l] < 0) continue;
-        float coef = a.weights ? a.weights[l] : 1.0f;
-        if (a.seg_scale) coef = __fmul_rn(coef, a.seg_scale[l]);
-        g = __fadd_rn(g, __fmul_rn(gbuf[(int64_t)e * sl.out_stride + sl.out_col + col], coef));
+    for (int c = c_first; c < used_chunks; c += a.or_chunks) {
+      const int s0 = c * bk::kOneRowChunk, s1 = min(sl.n_seg, s0 + bk::kOneRowChunk);
+      for (int col = 0; col < dim; ++col) {
+        float g = 0.f;
+        for (int e = s0 + threadIdx.x; e < s1; e += 256) {
+          const int64_t l = (int64_t)sl.seg_begin + e;
+          if (a.or_rows[l] < 0) continue;
+          float coef = a.weights ? a.weights[l] : 1.0f;
+          if (a.seg_scale) coef = __fmul_rn(coef, a.seg_scale[l]);
+          g = __fadd_rn(g, __fmul_rn(gbuf[(int64_t)e * sl.out_stride + sl.out_col + col], coef));
+        }
+        s_or_part[threadIdx.x] = g;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+          float tot = 0.f;
+          for (int q = 0; q < 256; ++q) tot = __fadd_rn(tot, s_or_part[q]);
+          __stcg(parts + (int64_t)c * dim + col, tot);
+        }
+        __syncthreads();
       }
-      s_or_part[threadIdx.x] = g;
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        float tot = 0.f;
-        for (int q = 0; q < 256; ++q) tot = __fadd_rn(tot, s_or_part[q]);
-        __stcg(a.or_partials + ((int64_t)f * a.or_chunks + c) * dim + col, tot);
-      }
-      __syncthreads();
     }
     __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) s_or_last = (atomicAdd(&a.or_tickets[f], 1) == used_chunks - 1);
+    if (threadIdx.x == 0) s_or_last = (atomicAdd(&a.or_tickets[f], 1) == used_ctas - 1);
     __syncthreads();
-    if (s_or_last && (int)threadIdx.x < dim) {
+    if (s_or_last) {
       __threadfence();
-      float tot = 0.f;
-      for (int q = 0; q < used_chunks; ++q)
-        tot = __fadd_rn(tot, __ldcg(a.or_partials + ((int64_t)f * a.or_chunks + q) * dim + threadIdx.x));
-      apply_scalar(a, row, (int)threadIdx.x, tot, 0);
+      const int64_t row = one_row_row(a, sl);
+      for (int col = threadIdx.x; col < dim && row >= 0; col += 256) {
+        float tot = 0.f;
+        for (int q = 0; q < used_chunks; ++q) tot = __fadd_rn(tot, __ldcg(parts + (int64_t)q * dim + col));
+        apply_scalar(a, (uint32_t)row, col, tot, 0);
+      }
     }
     __syncthreads();
     if (s_or_last && threadIdx.x == 0) a.or_tickets[f] = 0;
@@ -757,12 +785,13 @@ __global__ void __launch_bounds__(256) bwd_long_scalar_kernel(const __grid_const
       __syncthreads();
       if (threadIdx.x == 0) s_last = (atomicAdd(&a.run_done[qc.x], 1) == nch - 1);
       __syncthreads();
-      if (s_last && (int)threadIdx.x < a.dim) {
+      if (s_last) {
         __threadfence();
-        float tot = 0.f;
-        for (int c = 0; c < nch; ++c)
-          tot = __fadd_rn(tot, __ldcg(a.partials + (int64_t)(c0 + c) * a.dim + threadIdx.x));
-        apply_scalar(a, key, (int)threadIdx.x, tot, i);
+        for (int col = threadIdx.x; col < a.dim; col += 256) {
+          float tot = 0.f;
+          for (int c = 0; c < nch; ++c) tot = __fadd_rn(tot, __ldcg(a.partials + (int64_t)(c0 + c) * a.dim + col));
+          apply_scalar(a, key, col, tot, i);
+        }
       }
       __syncthreads();
     }
@@ -1023,37 +1052,42 @@ __device__ __forceinline__ void process_runs_scalar(const BwdArgs& a, const Slot
   __syncthreads();
   const int n = s_start[R];
   const int S_ENT = max(1, (kStageF4 * 4) / dim);
-  const int total = R * dim;
-  int idx = threadIdx.x;
-  float acc = 0.f;
-  for (int c0 = 0; c0 < n; c0 += S_ENT) {
-    const int c1 = min(n, c0 + S_ENT);
-    for (int q = threadIdx.x; q < (c1 - c0) * dim; q += THREADS) {
-      const int e = q / dim;
-      const uint32_t pos = (uint32_t)sp[c0 + e];
-      if (pos != kDonePos) {
-        float coef;
-        const float* src = grad_src(a, sv, pos, &coef);
-        s_stagef[q] = __fmul_rn(src[q - e * dim], coef);
+  // a thread walks its (run, column) items in order and keeps a run's partial sum across chunks; with more columns
+  // than threads two items of one thread could share a run, so the columns go in blocks of THREADS, one pass each
+  for (int cb = 0; cb < dim; cb += THREADS) {
+    const int width = min(THREADS, dim - cb);
+    const int total = R * width;
+    int idx = threadIdx.x;
+    float acc = 0.f;
+    for (int c0 = 0; c0 < n; c0 += S_ENT) {
+      const int c1 = min(n, c0 + S_ENT);
+      for (int q = threadIdx.x; q < (c1 - c0) * dim; q += THREADS) {
+        const int e = q / dim;
+        const uint32_t pos = (uint32_t)sp[c0 + e];
+        if (pos != kDonePos) {
+          float coef;
+          const float* src = grad_src(a, sv, pos, &coef);
+          s_stagef[q] = __fmul_rn(src[q - e * dim], coef);
+        }
       }
-    }
-    __syncthreads();
-    while (idx < total) {
-      const int r = idx / dim, c = idx - r * dim;
-      if (run_is_long(s_start, r)) {
+      __syncthreads();
+      while (idx < total) {
+        const int r = idx / width, c = cb + idx - r * width;
+        if (run_is_long(s_start, r)) {
+          idx += THREADS;
+          continue;
+        }
+        const int st = s_start[r], en = s_start[r + 1];
+        if (st >= c1) break;
+        const int lo = max(st, c0), hi = min(en, c1);
+        for (int i = lo; i < hi; ++i) acc = __fadd_rn(acc, s_stagef[(i - c0) * dim + c]);
+        if (en > c1) break;
+        apply_scalar(a, (uint32_t)(sp[st] >> 32), c, acc, 0);
+        acc = 0.f;
         idx += THREADS;
-        continue;
       }
-      const int st = s_start[r], en = s_start[r + 1];
-      if (st >= c1) break;
-      const int lo = max(st, c0), hi = min(en, c1);
-      for (int i = lo; i < hi; ++i) acc = __fadd_rn(acc, s_stagef[(i - c0) * dim + c]);
-      if (en > c1) break;
-      apply_scalar(a, (uint32_t)(sp[st] >> 32), c, acc, 0);
-      acc = 0.f;
-      idx += THREADS;
+      __syncthreads();
     }
-    __syncthreads();
   }
 }
 
@@ -1215,15 +1249,16 @@ __device__ __forceinline__ void warp_bucket_vec(const BwdArgs& a, const SlotView
   }
 }
 
-// dim == 1 (wide tables): a lane per run, the staged values are single floats
+// scalar rows - dim 1 (wide tables), and the warp-placed dims whose operands are not 16-byte aligned: a lane per run,
+// the staged values are single floats, one pass over the sorted chunks per column
 struct WarpSmem1 {
   float stage[32];
   float carry;
   uint32_t keys[32];
 };
 
-__device__ __forceinline__ void warp_bucket_d1(const BwdArgs& a, const SlotView& sv, const BkArgs& k, int b,
-                                               WarpSmem1* ws) {
+__device__ __forceinline__ void warp_bucket_scalar(const BwdArgs& a, const SlotView& sv, const BkArgs& k, int b,
+                                                   WarpSmem1* ws) {
   const int lane = threadIdx.x & 31;
   const int n = k.w.bcnt[b];
   if (n == 0 || n > bk::kWarpCap) return;
@@ -1235,51 +1270,54 @@ __device__ __forceinline__ void warp_bucket_d1(const BwdArgs& a, const SlotView&
     x[r] = q < n ? k.w.pairs[off + q] : ~0ull;
   }
   sort4(x, n <= 32 ? 32 : (n <= 64 ? 64 : 128), lane);
-  uint32_t carry_key = 0xFFFFFFFFu;
+#pragma unroll 1
+  for (int col = 0; col < a.dim; ++col) {
+    uint32_t carry_key = 0xFFFFFFFFu;
 #pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    if (r * 32 >= n) break;
-    const uint32_t key = (uint32_t)(x[r] >> 32), pos = (uint32_t)x[r];
-    const int nv = min(32, n - r * 32);
-    const uint32_t next_first = (r < 3 && (r + 1) * 32 < n) ? __shfl_sync(0xffffffffu, (uint32_t)(x[r < 3 ? r + 1 : 3] >> 32), 0)
-                                                            : 0xFFFFFFFFu;
-    uint32_t prevk = __shfl_up_sync(0xffffffffu, key, 1);
-    if (lane == 0) prevk = carry_key;
-    const bool is_head = lane < nv && key != prevk;
-    const unsigned H = __ballot_sync(0xffffffffu, is_head);
-    const int nh = __popc(H);
-    ws->keys[lane] = key;
-    const float open_sum = ws->carry;   // read before this chunk may overwrite it
-    if (lane < nv) {
-      float coef;
-      const float* src = grad_src(a, sv, pos, &coef);
-      ws->stage[lane] = __fmul_rn(src[0], coef);
+    for (int r = 0; r < 4; ++r) {
+      if (r * 32 >= n) break;
+      const uint32_t key = (uint32_t)(x[r] >> 32), pos = (uint32_t)x[r];
+      const int nv = min(32, n - r * 32);
+      const uint32_t next_first = (r < 3 && (r + 1) * 32 < n) ? __shfl_sync(0xffffffffu, (uint32_t)(x[r < 3 ? r + 1 : 3] >> 32), 0)
+                                                              : 0xFFFFFFFFu;
+      uint32_t prevk = __shfl_up_sync(0xffffffffu, key, 1);
+      if (lane == 0) prevk = carry_key;
+      const bool is_head = lane < nv && key != prevk;
+      const unsigned H = __ballot_sync(0xffffffffu, is_head);
+      const int nh = __popc(H);
+      ws->keys[lane] = key;
+      const float open_sum = ws->carry;   // read before this chunk may overwrite it
+      if (lane < nv) {
+        float coef;
+        const float* src = grad_src(a, sv, pos, &coef);
+        ws->stage[lane] = __fmul_rn(src[col], coef);
+      }
+      __syncwarp();
+      const uint32_t lastk = ws->keys[31];
+      const bool chunk_open = (nv == 32) && next_first == lastk;
+      const int lead = nh ? (__ffs(H) - 1) : nv;
+      if (lead > 0 && lane == 31) {   // (lane 31 never owns a head run of its own beyond the 32nd: see below)
+        float acc = open_sum;
+        for (int i = 0; i < lead; ++i) acc = __fadd_rn(acc, ws->stage[i]);
+        if (lead == 32 && chunk_open)
+          ws->carry = acc;
+        else
+          apply_scalar(a, carry_key, col, acc, 0);
+      }
+      if (lane < nh && !(lead > 0 && lane == 31)) {
+        const int h = __fns(H, 0, lane + 1);
+        const unsigned rest = (h == 31) ? 0u : (H >> (h + 1)) << (h + 1);
+        const int e_end = rest ? (__ffs(rest) - 1) : nv;
+        float acc = 0.f;
+        for (int i = h; i < e_end; ++i) acc = __fadd_rn(acc, ws->stage[i]);
+        if (e_end == 32 && chunk_open)
+          ws->carry = acc;
+        else
+          apply_scalar(a, ws->keys[h], col, acc, 0);
+      }
+      carry_key = chunk_open ? lastk : 0xFFFFFFFFu;
+      __syncwarp();
     }
-    __syncwarp();
-    const uint32_t lastk = ws->keys[31];
-    const bool chunk_open = (nv == 32) && next_first == lastk;
-    const int lead = nh ? (__ffs(H) - 1) : nv;
-    if (lead > 0 && lane == 31) {   // (lane 31 never owns a head run of its own beyond the 32nd: see below)
-      float acc = open_sum;
-      for (int i = 0; i < lead; ++i) acc = __fadd_rn(acc, ws->stage[i]);
-      if (lead == 32 && chunk_open)
-        ws->carry = acc;
-      else
-        apply_scalar(a, carry_key, 0, acc, 0);
-    }
-    if (lane < nh && !(lead > 0 && lane == 31)) {
-      const int h = __fns(H, 0, lane + 1);
-      const unsigned rest = (h == 31) ? 0u : (H >> (h + 1)) << (h + 1);
-      const int e_end = rest ? (__ffs(rest) - 1) : nv;
-      float acc = 0.f;
-      for (int i = h; i < e_end; ++i) acc = __fadd_rn(acc, ws->stage[i]);
-      if (e_end == 32 && chunk_open)
-        ws->carry = acc;
-      else
-        apply_scalar(a, ws->keys[h], 0, acc, 0);
-    }
-    carry_key = chunk_open ? lastk : 0xFFFFFFFFu;
-    __syncwarp();
   }
 }
 
@@ -1321,7 +1359,7 @@ __global__ void __launch_bounds__(bk::kThreads, ER_BK_MINB) bk_fused_kernel(cons
     if constexpr (LANES > 0 && LANES <= 8) {
       warp_bucket_vec<LANES>(a, sv, k, b, reinterpret_cast<WarpSmem<LANES>*>(p) + (threadIdx.x >> 5));
     } else if constexpr (LANES == 0) {
-      warp_bucket_d1(a, sv, k, b, reinterpret_cast<WarpSmem1*>(p) + (threadIdx.x >> 5));
+      warp_bucket_scalar(a, sv, k, b, reinterpret_cast<WarpSmem1*>(p) + (threadIdx.x >> 5));
     }
     return;
   }
@@ -1697,6 +1735,8 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
                  (uniq_rows == nullptr) == (n_uniq == nullptr),
              "uniq_rows, uniq_grads and n_uniq go together");
   ER_REQUIRE(dim > 0 && row_stride >= dim, "bad dim / row_stride");
+  // the CTA roles stage at least one whole gradient row in their kStageF4 * 4 floats of shared memory
+  ER_REQUIRE(dim <= kStageF4 * 4, "dim must be at most 4096");
   ER_REQUIRE(n_rows > 0 && n_rows < 0xFFFFFFFFLL, "n_rows must be in (0, 2^32-1)");
   ER_REQUIRE(n_slots > 0 && n_slots <= 2048, "n_slots must be in [1, 2048]");
   ER_REQUIRE(n_bufs > 0 && n_bufs <= ER_MAX_BUFS, "n_bufs must be in [1, ER_MAX_BUFS]");
@@ -1780,7 +1820,7 @@ static int embedding_bwd_impl(float* table, float* state0, float* state1, int64_
   a.or_rows = rows;
   a.or_partials = w.one_row_partials;
   a.or_tickets = w.tickets;
-  // one-row slots are single-valued: their segment count is the batch size, the smallest of the plan
+  // CTAs per one-row slot: enough for the average slot (a longer one is strided over, see one_row_cta)
   a.or_chunks = one_row ? (int)ceil_div(ceil_div(n_lookups_cap, (int64_t)n_slots), (int64_t)bk::kOneRowChunk) : 0;
   if (uniq_rows) {
     scan::exclusive_scan(HeadIn{w.keys, a.sentinel}, HeadOut{w.head_rank}, n_lookups_cap, n_uniq,

@@ -253,7 +253,10 @@ int er_embedding_fwd(const float* table, int64_t n_rows, int32_t dim,
  * row (even with a zero coefficient), so rows must already carry -1 for the
  * lookups safe_embedding_lookup_sparse prunes: er_bucketize_weighted given
  * the same weights does that.  state0/state1: adagrad accumulator | adam m, v (same
- * layout and stride as table; unused ones NULL).
+ * layout and stride as table; unused ones NULL).  dim is at most 4096.
+ * Rows, state and gradient buffers that are not 16-byte aligned (or a
+ * row_stride that is not a multiple of 4) take a scalar path with the same
+ * result as the aligned call wherever both sum in lookup order.
  * When uniq_rows/uniq_grads are non-NULL the deduplicated gradient is ALSO
  * written there (compact, sorted by row; *n_uniq receives the count); pass
  * table == NULL to only emit it. */
