@@ -327,7 +327,9 @@ class InputLayer(object):
         self.attention_modules[out_key] = att
         continue
       table = (f.embedding_name or fname + '_embedding') + ('_wide' if wide else '')
-      kind = 'tag' if f.kind == 'tag' else 'single'
+      # a RawFeature projection over raw_input_dim > 1 values is a fixed-length bag: ids 0..k-1 of every sample weighted
+      # by its k values and summed (input/input.py:648-673), so it goes through the multi-valued launch
+      kind = 'tag' if f.kind == 'tag' or (f.kind == 'raw' and f.raw_input_dim > 1) else 'single'
       # one output matrix per (group, launch kind): the single-valued and the CSR launch of a mixed group
       # write their own matrices, the group's concat is assembled from both in config order
       out_key = gname if kind == 'single' else gname + '#tag'
@@ -362,8 +364,10 @@ class InputLayer(object):
         assert T in (None, f.seq_len), 'hist_seq features of one group must share seq_len'
         T = f.seq_len
         table = f.embedding_name or '%s/%s_embedding' % (scope, h)
-        slot = self._add_slot(f.embedding_dim, sname + '/hist', h, table, 'seq')
-        hist.append(SeqColumn(h, f.embedding_dim, sname + '/hist', slot=slot))
+        # multi-valued histories run in a launch of their own: they write a matrix of their own too
+        out_key = sname + ('/mhist' if h in self.multi_valued_seq else '/hist')
+        slot = self._add_slot(f.embedding_dim, out_key, h, table, 'seq')
+        hist.append(SeqColumn(h, f.embedding_dim, out_key, slot=slot))
     self.seq_layout[sname] = lay = dict(key=key, hist=hist, T=T)
     return lay
 
@@ -425,7 +429,8 @@ class InputLayer(object):
           widths[slot.out_buf] += dim
           slots.append(slot)
         if sc.kind == 'tag':
-          cap = max_tag_lookups or 8 * B * len(slots)
+          raw = sum(self.features[fn].raw_input_dim for _, fn, _, _ in sc.items if self.features[fn].kind == 'raw')
+          cap = max_tag_lookups or 8 * B * len(slots) + B * raw
           sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=False, max_lookups=cap)
         elif sc.kind == 'mseq':
           cap = max_tag_lookups or 4 * B * sk[1] * len(slots)     # room for 4 values per step on average
@@ -433,6 +438,8 @@ class InputLayer(object):
         else:
           sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=True)
         for j, k in enumerate(keys):
+          # an output matrix belongs to one launch: lookup() finds each column's matrix by (dim, out_key)
+          assert (dim, k) not in self.out_index, 'output %s of width %d written by two launches' % (k, dim)
           self.out_index[(dim, k)] = (sk, j)
         if sc.kind == 'single':
           self.calls[dim] = sc.call
@@ -875,6 +882,8 @@ class InputLayer(object):
         # (values of every step back to back, steps per sample, values per (sample, step) - 0 beyond the length)
         ids, _, lens = features['seq_fea'][fname]
         w = None
+      elif self.features[fname].kind == 'raw':
+        ids, lens, w = self._raw_projection(fname, features)
       else:
         ids, lens, w = features['tag_fea'][fname]
       ids_list.append(ids)
@@ -897,6 +906,15 @@ class InputLayer(object):
     ids_cap = torch.zeros(cap, dtype=torch.int64, device=self.device)
     ids_cap[:L].copy_(ids)
     return ids_cap, lens, weights
+
+  def _raw_projection(self, fname, features):
+    """(ids, lens, weights) of a RawFeature projection over raw_input_dim k values: ids 0..k-1 of every sample,
+    weighted by its normalised values"""
+    c0, c1 = self.raw_cols[fname]
+    k, B = c1 - c0, self.batch_size
+    w = self.normalize_dense(features['dense_fea'])[:, c0:c1].reshape(-1)
+    ids = torch.arange(k, dtype=torch.int64, device=self.device).repeat(B)
+    return ids, torch.full((B,), k, dtype=torch.int32, device=self.device), w
 
   def has_group(self, group_name):
     return group_name in self.group_layout or group_name in self.seq_layout
