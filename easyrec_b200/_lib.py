@@ -36,6 +36,8 @@ OPT_SGD, OPT_ADAGRAD, OPT_LAZY_ADAM, OPT_ADAM_ROWS, OPT_MOMENTUM = 0, 1, 2, 3, 4
 ACT_GELU, ACT_LEAKY_RELU, ACT_ELU, ACT_SELU, ACT_TANH, ACT_SWISH, ACT_SIGMOID = 1, 2, 3, 4, 5, 6, 7
 MAX_BUFS = 8
 ABI_VERSION = 3
+KV_EMPTY = -1                 # ER_KV_EMPTY: a free slot of a key-value table's index
+KV_BUCKETS = 2**63 - 1        # the bucket count of a key-value table's slots: K1 then writes the 63-bit key
 CRITEO_N_DENSE, CRITEO_N_CAT = 13, 26   # ER_CRITEO_N_DENSE / ER_CRITEO_N_CAT: values per sample of a binary part
 HYPER_LR, HYPER_BETA1_POWER, HYPER_BETA2_POWER, HYPER_GRAD_SCALE, HYPER_N = 0, 1, 2, 3, 4
 
@@ -103,6 +105,10 @@ SIGNATURES = {
     'er_fingerprint64_i64': (c_i32, [c_vp, c_i64, c_vp]),
     'er_binary_unpack': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'er_load_embed': (c_i32, [ctypes.c_char_p, ctypes.c_char_p, c_i32, c_i32, c_i32, c_i64, c_vp, c_vp]),
+    'er_kv_find_or_insert': (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp,
+                                     c_i64, c_i32, c_f32, ctypes.c_uint64, c_f32, c_i32, c_vp]),
+    'er_kv_find': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_i64, c_vp, c_vp]),
+    'er_kv_insert_rows': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
     'er_embedding_fwd': (c_i32, [
         c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp,
         c_i32, ctypes.POINTER(c_vp), c_i32, c_vp, c_vp

@@ -15,12 +15,29 @@ _OPT_KIND = {'adagrad_optimizer': _lib.OPT_ADAGRAD, 'lazy_adam_optimizer': _lib.
              'adam_optimizer': _lib.OPT_ADAM_ROWS, 'momentum_optimizer': _lib.OPT_SGD}
 
 
+def ev_params(pipeline_config, fc):
+  """the EVParams of a feature: its own, else the model's (feature_column/feature_column.py:600-650), else None"""
+  if fc.HasField('ev_params'):
+    return fc.ev_params
+  mc = pipeline_config.model_config
+  return mc.ev_params if mc.HasField('ev_params') else None
+
+
 def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
   """FeatureConfig protos -> FeatureSpec list (config order = packed feature order)."""
   specs = []
   field_types = input_field_types(pipeline_config)
   for fc in config_util.get_feature_configs(pipeline_config):
     name = fc.feature_name if fc.HasField('feature_name') else fc.input_names[0]
+    ev = ev_params(pipeline_config, fc)
+    # a key-value table (ev_params): a pool of max_capacity rows per rank, filled as keys are trained
+    kv = int(ev.max_capacity) if ev is not None else 0
+    if kv and ftype_name(fc) == 'RawFeature' and fc.embedding_dim == 0 and raw_boundaries(fc) is None:
+      kv = 0   # a numeric column without a table: ev_params has nothing to apply to
+    if kv and (ftype_name(fc) not in ('IdFeature', 'TagFeature') or raw_boundaries(fc) is not None or
+               (fc.hash_bucket_size <= 0 and fc.num_buckets <= 0)):
+      raise NotImplementedError('feature %s: ev_params (key-value tables) on a %s; only IdFeatures and TagFeatures '
+                                'with hash_bucket_size or num_buckets take key-value tables' % (name, ftype_name(fc)))
     # a STRING field is hashed where its bytes are, by the reader (Fingerprint64 % hash_bucket_size); integer
     # fields go to the device as int64 and are hashed there from their decimal text (input/input.py:541-543)
     host_hashed = fc.hash_bucket_size > 0 and field_types.get(fc.input_names[0]) == 'STRING'
@@ -37,7 +54,8 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
     if ftype == 'IdFeature':
       specs.append(IL.id_feature(name, fc.embedding_dim, hash_bucket_size=fc.hash_bucket_size,
                                  num_buckets=fc.num_buckets, combiner=fc.combiner,
-                                 embedding_name=fc.embedding_name, packed_mod=packed_mod, host_hashed=host_hashed))
+                                 embedding_name=fc.embedding_name, packed_mod=packed_mod, host_hashed=host_hashed,
+                                 kv_capacity=kv))
     elif ftype == 'ComboFeature':
       # crossed_column over the inputs' string forms (feature_column/feature_column.py:424-455): the reader computes
       # FingerprintCat64 over the inputs' fingerprints % hash_bucket_size (readers.cross_hash); an id slot from there on
@@ -67,7 +85,7 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
                                     combiner=fc.combiner, embedding_name=fc.embedding_name,
                                     seq_len=((fc.max_seq_len if fc.HasField('max_seq_len') else default_seq_len)
                                              if ftype == 'SequenceFeature' else 1),
-                                    packed_mod=packed_mod, host_hashed=host_hashed))
+                                    packed_mod=packed_mod, host_hashed=host_hashed, kv_capacity=kv))
     else:
       raise NotImplementedError('feature_type %s (feature %s) is outside the hot-path scope' % (ftype, name))
   return specs
@@ -222,6 +240,20 @@ def check_scope(pipeline_config):
   mc = pipeline_config.model_config
   tc = pipeline_config.train_config
   bad = []
+  # EVParams first: PAI-TF's admission and eviction, and SOK's cache, cannot be pinned here
+  evs = [('model_config.ev_params', mc.ev_params)] if mc.HasField('ev_params') else []
+  for fc in config_util.get_feature_configs(pipeline_config):
+    if fc.HasField('ev_params'):
+      evs.append(('feature %s: ev_params' % (fc.feature_name if fc.HasField('feature_name') else fc.input_names[0]),
+                  fc.ev_params))
+  for path, ev in evs:
+    for field, on, why in (('filter_freq', ev.filter_freq > 0, 'admission by frequency'),
+                           ('steps_to_live', ev.steps_to_live > 0, 'eviction'),
+                           ('use_cache', ev.use_cache, 'the SOK embedding cache')):
+      if on:
+        bad.append('%s.%s (%s)' % (path, field, why))
+    if ev.max_capacity <= 0:
+      bad.append('%s.max_capacity 0' % path)
   dc = pipeline_config.data_config
   if dc.HasField('sample_weight') and mc.model_class in ('DSSM', 'MatchModel'):
     bad.append('data_config.sample_weight with a match model (the list-wise loss normalises by mean(w))')
@@ -237,8 +269,6 @@ def check_scope(pipeline_config):
     names = g.DESCRIPTOR.fields_by_name['wide_deep'].enum_type.values_by_number
     if names[g.wide_deep].name == 'WIDE_AND_DEEP':
       bad.append('feature_groups[%s].wide_deep WIDE_AND_DEEP' % g.group_name)
-  if mc.HasField('ev_params'):
-    bad.append('model_config.ev_params (embedding variables / dynamic tables)')
   if len(mc.kd) > 0:
     bad.append('model_config.kd (knowledge distillation losses)')
   if mc.HasField('variational_dropout'):
@@ -304,6 +334,12 @@ def build_model(pipeline_config, batch_size, device, generator=None, cpu_generat
   # input/parquet_input_v2.py:96-100) where the feature-column path maps out-of-range ids to 0
   specs = feature_specs(pipeline_config, packed_mod=input_type_name(pipeline_config).startswith('Parquet'),
                         default_seq_len=default_seq_len)
+  kv = [s.name for s in specs if s.kv_capacity]
+  if kv and world > 1 and not shard_tables:
+    raise NotImplementedError(
+        'ev_params (key-value tables) of %s with tables replicated over %d data-parallel ranks: replicas would need each '
+        'rank\'s gathered update translated to its own rows; train them row-sharded (train_distribute: '
+        'EmbeddingParallelStrategy) or on one GPU' % (kv, world))
   groups = feature_groups(mc)
   specs, keras_tables, pad_tags = embedding_layer_tables(mc, specs)
   opt = optimizer_settings(pipeline_config)
@@ -326,7 +362,9 @@ def build_model(pipeline_config, batch_size, device, generator=None, cpu_generat
                                     fc.sequence_combiner.WhichOneof('combiner')
                                     for fc in config_util.get_feature_configs(pipeline_config)
                                     if fc.HasField('sequence_combiner')},
-                     seq_output_groups=seq_groups)
+                     seq_output_groups=seq_groups,
+                     kv_seed=cpu_generator.initial_seed() if cpu_generator is not None else 0,
+                     kv_embedding_parallel=embedding_parallel(pipeline_config) or shard_tables)
   il.pad_tags = pad_tags   # tag features of a backbone `embedding_layer` block: the readers pad them with the bucket of ''
   # RawFeature.normalizer_fn: applied to the min-max normalised value on the device (input/input.py:642-646); the
   # readers apply the same function on the host to raw features they bucketize themselves (readers.bucketize_raw)

@@ -78,3 +78,70 @@ def restore_arena(arena, ckpt_path, scope='input_layer'):
   for name, view in _arena_vars(arena, scope):
     part = load_embed(ckpt_path, name, arena.dim, view.shape[0], arena.shard_rank, arena.shard_n)
     view.copy_(torch.from_numpy(part))
+
+
+def kv_part_path(ckpt_path, var_name, part, ext):
+  """a key-value variable's part: `.key` (int64 keys) or `.val` (fp32 [n, dim] rows in key order)
+  (compat/embedding_parallel_saver.py:187-220)"""
+  return '%s-embedding/embed-%s-part-%d.%s' % (ckpt_path, var_name.replace('/', '__'), part, ext)
+
+
+def save_kv_arena(arena, ckpt_path, scope='input_layer'):
+  """every variable of a key-value table's arena (the table and its optimizer slots) as this rank's `.key` / `.val`
+  parts: the keys that hold a row, and their rows; rank 0 removes the parts of a run with more workers.  Returns the
+  files written."""
+  keys, rows = arena.kv.items()
+  k = keys.numpy().astype(np.int64)
+  files = []
+  for name, view in _arena_vars(arena, scope):
+    kp, vp = (kv_part_path(ckpt_path, name, arena.shard_rank, e) for e in ('key', 'val'))
+    os.makedirs(os.path.dirname(kp), exist_ok=True)
+    with open(kp, 'wb') as f:
+      f.write(k.tobytes())
+    with open(vp, 'wb') as f:
+      f.write(np.ascontiguousarray(view[rows.to(view.device)].cpu().numpy(), np.float32).tobytes())
+    files += [kp, vp]
+    if arena.shard_rank == 0:
+      for old in glob.glob(kv_part_path(ckpt_path, name, 0, 'key').replace('-part-0.key', '-part-*.key')):
+        if _part_id(old) >= arena.shard_n:
+          os.remove(old)
+          if os.path.exists(old[:-4] + '.val'):
+            os.remove(old[:-4] + '.val')
+  return files
+
+
+def load_kv(ckpt_path, var_name, dim, rank, world):
+  """(keys int64 [n], vals fp32 [n, dim]): the keys with key % world == rank from every part on disk, in part order, as
+  load_kv_embed.cc assigns them (ops/src/load_kv_embed.cc:60-130)"""
+  pattern = kv_part_path(ckpt_path, var_name, 0, 'key').replace('-part-0.key', '-part-*.key')
+  ks, vs = [], []
+  for kp in sorted(glob.glob(pattern), key=_part_id):
+    k = np.fromfile(kp, np.int64)
+    v = np.fromfile(kp[:-4] + '.val', np.float32)
+    if v.size != k.size * dim:
+      raise ValueError('%s: %d values for %d keys of dim %d' % (kp[:-4] + '.val', v.size, k.size, dim))
+    mine = k % world == rank
+    ks.append(k[mine])
+    vs.append(v.reshape(-1, dim)[mine])
+  if not ks:
+    raise FileNotFoundError('no key-value parts %s' % pattern)
+  return np.concatenate(ks), np.concatenate(vs)
+
+
+def restore_kv_arena(arena, ckpt_path, scope='input_layer'):
+  """refill a key-value table's arena from the `.key` / `.val` parts of a run with any worker count: this rank keeps
+  the keys with key % N == rank; the index is rebuilt by the bulk-insert kernel"""
+  kv = arena.kv
+  keys = None
+  for name, view in _arena_vars(arena, scope):
+    k, v = load_kv(ckpt_path, name, arena.dim, arena.shard_rank, arena.shard_n)
+    if keys is None:
+      keys = k
+      if k.size > kv.capacity:
+        raise ValueError('key-value table %s: %d keys in the checkpoint exceed max_capacity %d'
+                         % (kv.name, k.size, kv.capacity))
+      view.zero_()
+    elif not np.array_equal(k, keys):
+      raise ValueError('%s: its keys differ from the table\'s' % name)
+    view[:k.size].copy_(torch.from_numpy(v))
+  kv.load(torch.from_numpy(keys), torch.arange(keys.size, dtype=torch.int64))

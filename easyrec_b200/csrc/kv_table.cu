@@ -1,0 +1,235 @@
+// Key-value embedding tables (ev_params): an open-addressing index from 63-bit keys to rows of a preallocated pool.
+//
+// The reference's counterparts are PAI-TF EmbeddingVariables on one worker and a SOK DynamicVariable under
+// EmbeddingParallelStrategy (compat/feature_column/feature_column.py:425-503): a row exists only for a key that has
+// been looked up, and two keys never share one.  Here K1 already produces the key (bucket count 2^63 - 1); these kernels
+// translate keys into pool rows, and K2 / K7 read and update those rows as any arena row.
+//
+// Index layout: keys[n_index] (ER_KV_EMPTY = free) and rows[n_index], n_index a power of two >= 16.  A key's probe
+// sequence is the 16-slot (128-byte) groups g, g + 1, ... from g = mix(key) mod (n_index / 16); a 16-lane tile loads
+// one group per step and compares all 16 keys with one ballot.  Slots are claimed with a 64-bit atomicCAS and never
+// freed, so every thread that looks up one key walks the same slots, sees each one's final value (either in its load or
+// as its CAS result), and stops on the same slot.  No thread ever waits for another thread's store: the claim launch
+// hands each new key a pool row and initialises it, and a second launch reads the row of every lookup's slot.
+#include "common.cuh"
+
+namespace er {
+
+constexpr int kKvTile = 16;
+constexpr int kKvThreads = 256;
+
+__device__ __forceinline__ uint64_t kv_mix(uint64_t z) {   // splitmix64 finaliser
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+struct KvIndex {
+  long long* keys;
+  int64_t* rows;
+  int64_t n_groups;   // n_index / 16, a power of two
+};
+
+// The slot of `k`, or -1 (find: absent; insert: every slot holds another key).  Uniform over the tile.  `won`: this
+// call claimed the slot.  A key is claimed whether or not the pool has a row left for it, so every lookup of one key
+// lands on the same slot; the claimer decides the row.
+template <bool kInsert>
+__device__ __forceinline__ int64_t kv_probe(const KvIndex& ix, int64_t k, int t, int base, unsigned tmask, bool& won) {
+  won = false;
+  const int64_t gmask = ix.n_groups - 1;
+  const int64_t g0 = (int64_t)(kv_mix((uint64_t)k) & (uint64_t)gmask);
+  for (int64_t i = 0; i < ix.n_groups; ++i) {
+    const int64_t s0 = ((g0 + i) & gmask) * kKvTile;
+    const long long v = *(volatile const long long*)(ix.keys + s0 + t);
+    const unsigned hit = (__ballot_sync(tmask, v == (long long)k) >> base) & 0xFFFFu;
+    if (hit) return s0 + __ffs(hit) - 1;
+    unsigned empty = (__ballot_sync(tmask, v == (long long)ER_KV_EMPTY) >> base) & 0xFFFFu;
+    if constexpr (!kInsert) {
+      if (empty) return -1;   // a key is never stored past a free slot of its sequence
+    } else {
+      while (empty) {
+        const int j = __ffs(empty) - 1;
+        long long old = 0;
+        if (t == j) old = atomicCAS((unsigned long long*)(ix.keys + s0 + j), (unsigned long long)ER_KV_EMPTY,
+                                    (unsigned long long)k);
+        old = __shfl_sync(tmask, old, base + j);
+        if (old == (long long)ER_KV_EMPTY) {
+          won = true;
+          return s0 + j;
+        }
+        if (old == (long long)k) return s0 + j;
+        empty &= empty - 1;   // another key took it: the next free slot of this group
+      }
+    }
+  }
+  return -1;
+}
+
+// The initial value of column c of key k's row: a normal(0, stddev), truncated at 2 stddev when `truncated`, drawn by
+// inverting the normal CDF at a uniform from a counter-based hash of (seed, key, column).  Independent of insertion
+// order, batch order and world size.
+__device__ __forceinline__ float kv_init_value(uint64_t seed, int64_t k, int c, float stddev, int truncated) {
+  const uint64_t h = kv_mix(seed ^ ((uint64_t)k * 0xD1B54A32D192ED03ull));
+  const uint64_t bits = kv_mix(h + (uint64_t)(c + 1) * 0x9E3779B97F4A7C15ull);
+  const double u = ((double)(bits >> 11) + 0.5) * 0x1.0p-53;
+  // Phi(-2) + u * (Phi(2) - Phi(-2)) for the truncated normal
+  const double p = truncated ? 0.022750131948179195 + u * 0.9544997361036416 : u;
+  return (float)(normcdfinv(p) * (double)stddev);
+}
+
+// the global key of a lookup: a row-sharded table's owner receives key div N and is rank key mod N
+__device__ __forceinline__ int64_t kv_global(int64_t k, int shard_n, int shard_rank) {
+  return k < 0 ? -1 : k * shard_n + shard_rank;
+}
+
+struct KvInit {
+  float* weight;
+  float* state0;
+  float* state1;
+  int64_t row_stride;
+  int dim;
+  float state0_init;
+  uint64_t seed;
+  float stddev;
+  int truncated;
+};
+
+__global__ void __launch_bounds__(kKvThreads)
+    kv_claim_kernel(KvIndex ix, int64_t capacity, unsigned long long* stats, const int64_t* __restrict__ keys, int64_t n,
+                    int shard_n, int shard_rank, int64_t* __restrict__ slots, KvInit in) {
+  const int lane = threadIdx.x & 31, t = lane & (kKvTile - 1), base = lane & kKvTile;
+  const unsigned tmask = 0xFFFFu << base;
+  const int64_t n_tiles = (int64_t)gridDim.x * (blockDim.x / kKvTile);
+  for (int64_t l = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kKvTile; l < n; l += n_tiles) {
+    const int64_t k = kv_global(keys[l], shard_n, shard_rank);
+    bool won = false;
+    const int64_t s = k >= 0 ? kv_probe<true>(ix, k, t, base, tmask, won) : -1;
+    if (won) {
+      unsigned long long r = 0;
+      if (t == 0) r = atomicAdd(stats, 1ull);
+      r = __shfl_sync(tmask, r, base);
+      const int64_t row = r < (unsigned long long)capacity ? (int64_t)r : -1;
+      if (t == 0) ix.rows[s] = row;
+      if (row >= 0) {
+        const int64_t o = row * in.row_stride;
+        for (int c = t; c < in.dim; c += kKvTile) {
+          in.weight[o + c] = kv_init_value(in.seed, k, c, in.stddev, in.truncated);
+          if (in.state0) in.state0[o + c] = in.state0_init;
+          if (in.state1) in.state1[o + c] = 0.f;
+        }
+      }
+    }
+    if (t == 0) slots[l] = s;
+  }
+}
+
+// slots[l] -> the pool row of its key (in place); a live lookup left without a row counts in stats[1]
+__global__ void __launch_bounds__(kKvThreads)
+    kv_resolve_kernel(const int64_t* __restrict__ index_rows, unsigned long long* stats,
+                      const int64_t* __restrict__ keys, int64_t n, int64_t* __restrict__ rows) {
+  for (int64_t l = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; l < n; l += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t s = rows[l];
+    const int64_t r = s >= 0 ? index_rows[s] : -1;
+    rows[l] = r;
+    if (r < 0 && keys[l] >= 0) atomicAdd(stats + 1, 1ull);
+  }
+}
+
+__global__ void __launch_bounds__(kKvThreads)
+    kv_find_kernel(KvIndex ix, const int64_t* __restrict__ keys, int64_t n, int shard_n, int shard_rank,
+                   int64_t zero_row, int64_t* __restrict__ rows) {
+  const int lane = threadIdx.x & 31, t = lane & (kKvTile - 1), base = lane & kKvTile;
+  const unsigned tmask = 0xFFFFu << base;
+  const int64_t n_tiles = (int64_t)gridDim.x * (blockDim.x / kKvTile);
+  for (int64_t l = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kKvTile; l < n; l += n_tiles) {
+    const int64_t k = kv_global(keys[l], shard_n, shard_rank);
+    bool won;
+    const int64_t s = k >= 0 ? kv_probe<false>(ix, k, t, base, tmask, won) : -1;
+    const int64_t r = s >= 0 ? ix.rows[s] : -1;
+    if (t == 0) rows[l] = k < 0 ? -1 : (r >= 0 ? r : zero_row);
+  }
+}
+
+__global__ void __launch_bounds__(kKvThreads)
+    kv_insert_rows_kernel(KvIndex ix, const int64_t* __restrict__ keys, const int64_t* __restrict__ given, int64_t n,
+                          unsigned long long* stats) {
+  const int lane = threadIdx.x & 31, t = lane & (kKvTile - 1), base = lane & kKvTile;
+  const unsigned tmask = 0xFFFFu << base;
+  const int64_t n_tiles = (int64_t)gridDim.x * (blockDim.x / kKvTile);
+  for (int64_t l = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / kKvTile; l < n; l += n_tiles) {
+    const int64_t k = keys[l];
+    bool won = false;
+    const int64_t s = k >= 0 ? kv_probe<true>(ix, k, t, base, tmask, won) : -1;
+    if (t == 0) {
+      if (won)
+        ix.rows[s] = given[l];
+      else
+        atomicAdd(stats + 1, 1ull);   // a negative, repeated or unplaceable key
+    }
+  }
+}
+
+inline int kv_grid(int64_t n, int per_cta) { return grid_for(n, per_cta, 8); }
+
+}  // namespace er
+
+#define ER_KV_REQUIRE_INDEX(keys, rows, n_index)                                                      \
+  ER_REQUIRE((keys) && (rows), "null index array");                                                   \
+  ER_REQUIRE((n_index) >= 16 && ((n_index) & ((n_index) - 1)) == 0, "n_index must be a power of two >= 16")
+
+extern "C" int er_kv_find_or_insert(int64_t* index_keys, int64_t* index_rows, int64_t n_index, int64_t capacity,
+                                    int64_t* stats, const int64_t* keys, int64_t n, int32_t shard_n, int32_t shard_rank,
+                                    int64_t* rows, float* weight, float* state0, float* state1, int64_t row_stride,
+                                    int32_t dim, float state0_init, uint64_t seed, float init_stddev,
+                                    int32_t init_truncated, er_stream_t stream) {
+  using namespace er;
+  ER_KV_REQUIRE_INDEX(index_keys, index_rows, n_index);
+  ER_REQUIRE(stats && weight, "null stats or weight array");
+  ER_REQUIRE(n >= 0 && (n == 0 || (keys && rows)), "null keys or rows");
+  ER_REQUIRE((const void*)keys != (const void*)rows, "keys and rows must not alias");
+  ER_REQUIRE(capacity > 0 && 2 * capacity <= n_index, "n_index must be at least twice the capacity");
+  ER_REQUIRE(dim > 0 && row_stride >= dim, "dim must be positive and row_stride >= dim");
+  ER_REQUIRE(shard_n > 0 && shard_rank >= 0 && shard_rank < shard_n, "shard_rank must be in [0, shard_n)");
+  if (n == 0) return ER_OK;
+  const KvIndex ix{(long long*)index_keys, index_rows, n_index / kKvTile};
+  const KvInit in{weight, state0, state1, row_stride, dim, state0_init, seed, init_stddev, init_truncated != 0};
+  cudaStream_t st = as_stream(stream);
+  kv_claim_kernel<<<kv_grid(n, kKvThreads / kKvTile), kKvThreads, 0, st>>>(ix, capacity, (unsigned long long*)stats,
+                                                                            keys, n, shard_n, shard_rank, rows, in);
+  kv_resolve_kernel<<<kv_grid(n, kKvThreads), kKvThreads, 0, st>>>(index_rows, (unsigned long long*)stats, keys, n,
+                                                                   rows);
+  count_launches(2);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_kv_find(const int64_t* index_keys, const int64_t* index_rows, int64_t n_index, const int64_t* keys,
+                          int64_t n, int32_t shard_n, int32_t shard_rank, int64_t zero_row, int64_t* rows,
+                          er_stream_t stream) {
+  using namespace er;
+  ER_KV_REQUIRE_INDEX(index_keys, index_rows, n_index);
+  ER_REQUIRE(shard_n > 0 && shard_rank >= 0 && shard_rank < shard_n, "shard_rank must be in [0, shard_n)");
+  ER_REQUIRE(n >= 0 && (n == 0 || (keys && rows)), "null keys or rows");
+  if (n == 0) return ER_OK;
+  const KvIndex ix{(long long*)index_keys, (int64_t*)index_rows, n_index / kKvTile};
+  kv_find_kernel<<<kv_grid(n, kKvThreads / kKvTile), kKvThreads, 0, as_stream(stream)>>>(ix, keys, n, shard_n, shard_rank, zero_row, rows);
+  count_launches(1);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_kv_insert_rows(int64_t* index_keys, int64_t* index_rows, int64_t n_index, const int64_t* keys,
+                                 const int64_t* rows, int64_t n, int64_t* stats, er_stream_t stream) {
+  using namespace er;
+  ER_KV_REQUIRE_INDEX(index_keys, index_rows, n_index);
+  ER_REQUIRE(stats, "null stats array");
+  ER_REQUIRE(n >= 0 && (n == 0 || (keys && rows)), "null keys or rows");
+  ER_REQUIRE(2 * n <= n_index, "more keys than half the index");
+  if (n == 0) return ER_OK;
+  const KvIndex ix{(long long*)index_keys, index_rows, n_index / kKvTile};
+  kv_insert_rows_kernel<<<kv_grid(n, kKvThreads / kKvTile), kKvThreads, 0, as_stream(stream)>>>(
+      ix, keys, rows, n, (unsigned long long*)stats);
+  count_launches(1);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}

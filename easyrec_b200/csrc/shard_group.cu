@@ -9,7 +9,7 @@
 //        pos[l]                 = o * cap + k of lookup l's row (-1 = dropped / over capacity)
 //        counts[o]              = distinct rows owned by o (may exceed cap: then counts[N] counts the lost lookups)
 //
-// Dedup by an open-addressing table in the workspace (keys = owner<<48 | row, linear probing, 64-bit CAS):
+// Dedup by an open-addressing table in the workspace (keys = row * N + owner, linear probing, 64-bit CAS):
 // 2 x n entries of 8 B + 4 B, L2 resident at batch sizes (5 MB at 213K lookups).  Which k a row gets depends on
 // the order of the atomics; no result depends on it: the forward reads rows through pos[], the requester sums
 // duplicate lookups of a position in lookup order, and the owner sees a row at most once per source rank and sums
@@ -57,7 +57,9 @@ __global__ void __launch_bounds__(256) insert_kernel(Args a) {
     const int64_t r = in ? a.row[l] : -1;
     const int32_t o = in ? a.owner[l] : -1;
     const bool live = r >= 0 && o >= 0 && o < a.world;
-    const unsigned long long key = ((unsigned long long)o << 48) | (unsigned long long)r;
+    // (row, owner) -> row * world + owner: one-to-one for every row below 2^63 / world, which covers the 63-bit keys of
+    // a key-value table (row = key div N, owner = key mod N) as well as arena rows
+    const unsigned long long key = (unsigned long long)r * (unsigned long long)a.world + (unsigned long long)o;
     // lookups of one slot are neighbours and hot ids (one-row tables, the head of a Zipf distribution) repeat
     // thousands of times per batch: one lane per distinct key of the warp talks to the table, the rest copy its answer
     const unsigned peers = __match_any_sync(0xffffffffu, live ? key : (kEmpty - (unsigned)lane));

@@ -49,16 +49,18 @@ class Arena(object):
     self.shard_rank = shard_rank
     self.tables = {}   # name -> (row_offset, n_rows_local, n_rows_global)
     self.n_rows = 0
+    self.kv = None     # KvTable: the arena holds one key-value table
     self.weight = None
     self.state0 = None
     self.state1 = None
 
-  def add_table(self, name, n_rows_global):
+  def add_table(self, name, n_rows_global, local_rows=None):
+    """local_rows: this rank's rows when they are not a share of n_rows_global (a key-value table's pool)"""
     if name in self.tables:
       assert self.tables[name][2] == n_rows_global, 'shared table %s: size mismatch' % name
       return
     # per-worker rows (V + N - 1) // N  (feature_column.py:461-463)
-    local = (n_rows_global + self.shard_n - 1) // self.shard_n
+    local = (n_rows_global + self.shard_n - 1) // self.shard_n if local_rows is None else local_rows
     self.tables[name] = (self.n_rows, local, n_rows_global)
     self.n_rows += local
 
@@ -90,6 +92,7 @@ class Arena(object):
       del tmp
     self.weight = w
     self.opt_kind = opt_kind
+    self.adagrad_init = adagrad_init
 
     def state(i, fill):
       if interleave:
@@ -108,13 +111,92 @@ class Arena(object):
       self.state0 = state(0, 0.0)
       self.state1 = state(1, 0.0)
     # tf.train.AdamOptimizer decays m, v and moves w on EVERY row each step; the rows of this step's lookups are
-    # marked here so that the dense sweep skips exactly the rows the fused row update has already written
+    # marked here so that the dense sweep skips exactly the rows the fused row update has already written.  A
+    # key-value table has no sweep: both of the reference's paths apply _apply_sparse to the gathered rows only
+    # (compat/sok_optimizer.py:215-276, and EmbeddingVariable's sparse apply on one worker)
     self.touched = (torch.zeros(self.n_rows, dtype=torch.uint8, device=self.device)
-                    if opt_kind == _lib.OPT_ADAM_ROWS else None)
+                    if opt_kind == _lib.OPT_ADAM_ROWS and self.kv is None else None)
 
   def table_view(self, name):
     off, n, _ = self.tables[name]
     return self.weight[off:off + n]
+
+
+def _mix64(z):
+  """splitmix64's finaliser on a python int"""
+  m = 2**64 - 1
+  z &= m
+  z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & m
+  z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & m
+  return z ^ (z >> 31)
+
+
+class KvTable(object):
+  """A key-value table (ev_params) on an arena of its own: `capacity` pool rows, then one zero row that evaluation reads
+  for keys it has not seen.  The open-addressing index and its counters live on the device (csrc/kv_table.cu); the
+  slots of the table have num_buckets = KV_BUCKETS, so K1 hands over keys, which lookup() turns into pool rows."""
+
+  def __init__(self, name, arena, capacity, seed, embedding_parallel=False):
+    self.name = name
+    self.arena = arena
+    self.capacity = int(capacity)
+    self.zero_row = self.capacity
+    n_index = 16
+    while n_index < 2 * self.capacity:
+      n_index *= 2
+    dev = arena.device
+    self.index_keys = torch.full((n_index,), _lib.KV_EMPTY, dtype=torch.int64, device=dev)
+    self.index_rows = torch.full((n_index,), -1, dtype=torch.int64, device=dev)
+    self.stats = torch.zeros(2, dtype=torch.int64, device=dev)   # rows handed out, lookups left without a row
+    # initial rows depend on (seed, table, key) only: the table's name enters through its fingerprint
+    self.seed = _mix64(int(seed) ^ _lib.fingerprint64(name))
+    # one worker: the column's initializer, the truncated normal Arena.materialize draws for static tables;
+    # EmbeddingParallelStrategy: the DynamicVariable's `random {"stddev": 0.0025}` (feature_column.py:472-480), a
+    # normal(0, 0.0025)
+    self.init_truncated = not embedding_parallel
+    self.init_stddev = 0.0025 if embedding_parallel else 0.01 / math.sqrt(arena.dim)
+
+  def lookup(self, keys, rows, train):
+    """rows = the pool rows of `keys`: find-or-insert when training, find only (unseen keys -> the zero row) else.  On
+    a row-sharded arena `keys` are the owner-local keys (key div N) this rank received; the index holds global keys."""
+    a = self.arena
+    if train:
+      init0 = a.adagrad_init if a.opt_kind == _lib.OPT_ADAGRAD else 0.0
+      return K.kv_find_or_insert(self.index_keys, self.index_rows, self.capacity, self.stats, keys, rows,
+                                 a.weight, a.state0, a.state1, init0, self.seed, self.init_stddev, self.init_truncated,
+                                 shard_n=a.shard_n, shard_rank=a.shard_rank)
+    return K.kv_find(self.index_keys, self.index_rows, keys, self.zero_row, rows, shard_n=a.shard_n,
+                     shard_rank=a.shard_rank)
+
+  def size(self):
+    """keys that hold a row (reads the device counter back)"""
+    return min(int(self.stats[0]), self.capacity)
+
+  def check(self):
+    n, dropped = (int(v) for v in self.stats.cpu())
+    if dropped or n > self.capacity:
+      raise _lib.ErError('key-value table %s: more distinct keys than its max_capacity %d (ev_params); %d lookups had '
+                         'no row' % (self.name, self.capacity, dropped))
+
+  def items(self):
+    """(global keys, rows) of every key that holds a row, in row order (host tensors)"""
+    k, r = self.index_keys.cpu(), self.index_rows.cpu()
+    live = (k != _lib.KV_EMPTY) & (r >= 0)
+    k, r = k[live], r[live]
+    order = torch.argsort(r)
+    return k[order], r[order]
+
+  def load(self, keys, rows):
+    """rebuild the index from (keys, rows) with the bulk-insert kernel; the caller fills the pool rows"""
+    self.index_keys.fill_(_lib.KV_EMPTY)
+    self.index_rows.fill_(-1)
+    self.stats.zero_()
+    if keys.numel():
+      K.kv_insert_rows(self.index_keys, self.index_rows, keys.to(self.arena.device), rows.to(self.arena.device),
+                       self.stats)
+    self.stats[0] = keys.numel()
+    if int(self.stats[1]):
+      raise _lib.ErError('key-value table %s: restored keys are negative or repeated' % self.name)
 
 
 class ArenaCall(object):
@@ -189,7 +271,7 @@ def adam_dense_decay(arena, rows, opt, n_dev=None):
   """The dense half of tf.train.AdamOptimizer's sparse apply (builders/optimizer_builder.py:61-66; behaviour
   stated at compat/adam_s.py:74-81): every row WITHOUT a gradient this step still gets m *= b1, v *= b2,
   w -= lr_t*m/(sqrt(v)+eps).  `rows` are the step's looked-up rows (already updated by K7's row rule)."""
-  if arena.opt_kind != _lib.OPT_ADAM_ROWS:
+  if arena.opt_kind != _lib.OPT_ADAM_ROWS or arena.kv is not None:
     return
   if rows is not None and rows.numel():
     K.mark_rows(rows, arena.n_rows, arena.touched, 1, n_dev=n_dev)

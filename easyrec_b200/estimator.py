@@ -229,6 +229,7 @@ class EasyRecEstimator(object):
         if reader is not None:
           self.last_loss_value = reader.push(loss)
         if self.global_step % every == 0:
+          self.input_layer.check_kv()   # a key-value table that ran out of rows stops the run when the loss is logged
           dt = time.time() - t0
           logging.info('global_step = %d, loss = %.6f, global_step/sec = %.2f', self.global_step, float(loss),
                        (self.global_step - n0) / max(dt, 1e-9))
@@ -236,6 +237,7 @@ class EasyRecEstimator(object):
           break
     finally:
       stream.close()
+    self.input_layer.check_kv()
     if reader is not None and loss is not None:
       self.last_loss_value = reader.flush()      # the last step's loss: every step's result has reached the host
       return self.last_loss_value
@@ -372,6 +374,8 @@ class EasyRecEstimator(object):
     torch.save({'model': self.model.state_dict(),
                 'arenas': {d: a.storage for d, a in self.input_layer.arenas.items()},
                 'tables': {d: a.tables for d, a in self.input_layer.arenas.items()},
+                # key-value tables: the (key, pool row) pairs of their indexes
+                'kv': {d: a.kv.items() for d, a in self.input_layer.arenas.items() if a.kv is not None},
                 # dense optimizer slots (Adagrad accumulators | Adam m, v), keyed by parameter name: the reference's
                 # Saver stores every slot variable, a resumed run continues from them
                 'dense_slots': {n: [None if st is None else st[o:o + k].clone() for st in (do.s0, do.s1)]
@@ -380,7 +384,10 @@ class EasyRecEstimator(object):
                 'global_step': self.global_step}, path)
     if embedding_parts:
       for a in self.input_layer.arenas.values():
-        checkpoint.save_arena(a, path[:-3])
+        if a.kv is not None:
+          checkpoint.save_kv_arena(a, path[:-3])   # `.key` / `.val` parts
+        else:
+          checkpoint.save_arena(a, path[:-3])
     return path
 
   def restore(self, path):
@@ -402,11 +409,15 @@ class EasyRecEstimator(object):
             st[o:o + k].copy_(saved)
     parts = os.path.isdir(path[:-3] + '-embedding')
     for d, a in self.input_layer.arenas.items():
-      if parts:
+      if parts and a.kv is not None:
+        checkpoint.restore_kv_arena(a, path[:-3])
+      elif parts:
         checkpoint.restore_arena(a, path[:-3])
       else:
         assert ck['tables'][d] == a.tables, 'checkpoint was written with another table plan'
         a.storage.copy_(ck['arenas'][d])
+        if a.kv is not None:
+          a.kv.load(*ck['kv'][d])
     return self
 
 

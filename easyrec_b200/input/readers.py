@@ -263,7 +263,7 @@ class CSVInput(object):
       if fc.hash_bucket_size > 0 and self.ftypes.get(fc.input_names[0]) == 'STRING' and name in input_layer.features:
         assert input_layer.features[name].bucket_mode in (_lib.BUCKET_IDENTITY, _lib.BUCKET_MOD), \
             'feature %s: the table plan must take host-hashed buckets (builder.feature_specs)' % name
-        self.hash_buckets[name] = fc.hash_bucket_size
+        self.hash_buckets[name] = input_layer.features[name].num_buckets   # (2^63 - 1 for a key-value table)
 
   def _token(self, x, feature):
     """one id token -> int64: Fingerprint64 % hash_bucket_size for a host-hashed STRING field ('' -> -1, the

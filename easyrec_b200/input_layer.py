@@ -34,7 +34,9 @@ FeatureSpec = collections.namedtuple(
     'FeatureSpec',
     ['name', 'kind',            # 'id' | 'raw' | 'tag' | 'seq'
      'embedding_dim', 'bucket_mode', 'num_buckets', 'combiner', 'embedding_name',
-     'min_val', 'max_val', 'raw_input_dim', 'seq_len'])
+     'min_val', 'max_val', 'raw_input_dim', 'seq_len',
+     'kv_capacity'],            # > 0: a key-value table (ev_params) of that many rows per rank
+    defaults=(0,))
 
 
 def _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed=False):
@@ -49,13 +51,23 @@ def _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed=False):
   return _lib.BUCKET_IDENTITY, num_buckets
 
 
+def _kv_buckets(hash_bucket_size, num_buckets, kv_capacity):
+  """a key-value column hashes into the full 63-bit space: MAX_HASH_BUCKET_SIZE for hashed columns, sys.maxsize for
+  identity columns (feature_column/feature_column.py:19,250-256,288-291)"""
+  if not kv_capacity:
+    return hash_bucket_size, num_buckets
+  return (_lib.KV_BUCKETS, 0) if hash_bucket_size > 0 else (0, _lib.KV_BUCKETS)
+
+
 def id_feature(name, embedding_dim, hash_bucket_size=0, num_buckets=0, combiner='sum',
-               embedding_name='', packed_mod=False, host_hashed=False):
+               embedding_name='', packed_mod=False, host_hashed=False, kv_capacity=0):
   """IdFeature: hash_bucket_size -> Fingerprint64(as_string) % size; num_buckets -> identity
   (feature_column/feature_column.py:259-300).  packed_mod: the Parquet packed rule
-  `vals % num_buckets` (input/parquet_input.py:221)."""
+  `vals % num_buckets` (input/parquet_input.py:221).  kv_capacity > 0: a key-value table (ev_params) of that many
+  rows per rank instead of a fixed-size one."""
+  hash_bucket_size, num_buckets = _kv_buckets(hash_bucket_size, num_buckets, kv_capacity)
   mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed)
-  return FeatureSpec(name, 'id', embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1, 1)
+  return FeatureSpec(name, 'id', embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1, 1, int(kv_capacity))
 
 
 def raw_feature(name, embedding_dim=0, min_val=0.0, max_val=0.0, raw_input_dim=1):
@@ -69,14 +81,15 @@ def raw_feature(name, embedding_dim=0, min_val=0.0, max_val=0.0, raw_input_dim=1
 
 
 def multi_feature(name, kind, embedding_dim, hash_bucket_size=0, num_buckets=0, combiner='sum',
-                  embedding_name='', seq_len=1, packed_mod=False, host_hashed=False):
+                  embedding_name='', seq_len=1, packed_mod=False, host_hashed=False, kv_capacity=0):
   """TagFeature (kind 'tag': multi-valued, pooled by `combiner`, optional kv weights;
   feature_column/feature_column.py:301-360) or SequenceFeature (kind 'seq': un-pooled [B,T,D];
   feature_column_v2.py:4988-5002)."""
   assert kind in ('tag', 'seq')
+  hash_bucket_size, num_buckets = _kv_buckets(hash_bucket_size, num_buckets, kv_capacity)
   mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed)
   return FeatureSpec(name, kind, embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1,
-                     max(int(seq_len), 1))
+                     max(int(seq_len), 1), int(kv_capacity))
 
 
 _COMBINER = {'sum': _lib.COMBINER_SUM, 'mean': _lib.COMBINER_MEAN, 'sqrtn': _lib.COMBINER_SQRTN}
@@ -168,8 +181,13 @@ class InputLayer(object):
   def __init__(self, features, groups, batch_size, device, wide_output_dim=1,
                embedding_optimizer=_lib.OPT_ADAGRAD, shard_n=1, shard_rank=0, generator=None,
                adagrad_init=0.1, seq_att_groups=None, max_tag_lookups=None, uniform_tables=None,
-               dense_generator=None, multi_valued_seq=(), seq_combiners=None, seq_output_groups=()):
+               dense_generator=None, multi_valued_seq=(), seq_combiners=None, seq_output_groups=(), kv_seed=0,
+               kv_embedding_parallel=False):
     self.features = collections.OrderedDict((f.name, f) for f in features)
+    # key-value tables: initial rows from (kv_seed, table, key); kv_embedding_parallel: the config trains under
+    # EmbeddingParallelStrategy, whose DynamicVariables draw another distribution (embedding.KvTable)
+    self.kv_seed = int(kv_seed)
+    self.kv_embedding_parallel = bool(kv_embedding_parallel)
     # groups read only by backbone `input_layer { output_seq_and_normal_feature: true }` blocks
     # (layers/common_layers.py:104-131): their SequenceFeatures come out un-pooled as one [B, T, sum D] tensor
     self.seq_output_groups = set(seq_output_groups)
@@ -194,14 +212,16 @@ class InputLayer(object):
       c += self.features[n].raw_input_dim
     self.n_dense = c
     # ---- table plan -------------------------------------------------------------------
-    self.arenas = collections.OrderedDict()          # dim -> Arena
-    self.subcalls = collections.OrderedDict()        # dim -> OrderedDict(key -> _SubCall)
+    # arenas are keyed by their dim; a key-value table has an arena of its own, keyed (dim, table)
+    self.arenas = collections.OrderedDict()          # arena key -> Arena
+    self.subcalls = collections.OrderedDict()        # arena key -> OrderedDict(key -> _SubCall)
     self.group_layout = {}       # group -> [GroupColumn] in concat order
     self.seq_layout = {}         # seq group -> dict(key=[SeqColumn], hist=[SeqColumn], T=steps)
     self.seq_group_layout = {}   # output_seq_and_normal_feature group -> dict(seq=[SeqColumn], T=steps)
     self.attention_modules = collections.OrderedDict()
     self.seqc_order = {}      # group -> names of its sequence-combiner features in config order
     self._shard = (shard_n, shard_rank)
+    self._table_kv = {}       # (dim, table) -> the kv_capacity of its readers (0: a static table)
     for gname, g in groups.items():
       self._plan_group(gname, g, dense_generator)
     for sname, maps in self.seq_att_groups.items():
@@ -245,14 +265,32 @@ class InputLayer(object):
     self._pos = {}
     self._next_ids = {}
     self._clip_state = {}
+    self._kv_bufs = {}        # (arena key, launch) -> the pool rows of a key-value table's single-valued launch
 
   # ---- table plan: the constructor's stages ---------------------------------------------
   def _add_slot(self, dim, out_key, fname, table, kind, wide=False):
     """one lookup of feature `fname` from `table` into the (dim, out_key) output matrix; returns its Slot"""
     f = self.features[fname]
     B = self.batch_size
-    arena = self.arenas.setdefault(dim, E.Arena(dim, self.device, *self._shard))
-    arena.add_table(table, f.num_buckets)
+    ak = dim
+    if f.kv_capacity:
+      if kind == 'seq' or f.kind == 'raw':
+        raise NotImplementedError('ev_params (key-value table) on %s feature %s: only IdFeatures and TagFeatures take '
+                                  'key-value tables' % ('SequenceFeature' if kind == 'seq' else 'RawFeature', fname))
+      ak = (dim, table)
+      # every reader of a key-value table writes matrices of its own: (dim, out_key) names one launch's output
+      out_key = '%s#kv/%s' % (out_key, table)
+    if self._table_kv.setdefault((dim, table), f.kv_capacity) != f.kv_capacity:
+      raise ValueError('table %s: read by features with different ev_params (%s)' % (table, fname))
+    arena = self.arenas.get(ak)
+    if arena is None:
+      arena = self.arenas[ak] = E.Arena(dim, self.device, *self._shard)
+      if f.kv_capacity:
+        arena.kv = E.KvTable(table, arena, f.kv_capacity, self.kv_seed, self.kv_embedding_parallel)
+    if f.kv_capacity:
+      arena.add_table(table, f.kv_capacity + 1, local_rows=f.kv_capacity + 1)   # max_capacity rows per rank + zero row
+    else:
+      arena.add_table(table, f.num_buckets)
     if kind == 'seq' and fname in self.multi_valued_seq:
       kind = 'mseq'
       sk, nseg = ('mseq', f.seq_len), B * f.seq_len
@@ -262,11 +300,12 @@ class InputLayer(object):
       sk, nseg = ('tag',), B
     else:
       sk, nseg = ('single',), B
-    subs = self.subcalls.setdefault(dim, collections.OrderedDict())
+    subs = self.subcalls.setdefault(ak, collections.OrderedDict())
     sc = subs.setdefault(sk, _SubCall(sk[0], nseg))
     comb = _lib.COMBINER_SUM if (wide or f.kind == 'raw' or kind == 'seq') else _COMBINER[f.combiner]
     slot = E.Slot(out_key + '/' + fname, table, f.bucket_mode, f.num_buckets, comb, out_buf=out_key,
                   n_seg_per_sample=f.seq_len if kind in ('seq', 'mseq') else 1)
+    slot.out_key = out_key
     # id and sequence slots never carry per-lookup weights (raw-value and kv-weighted tag slots do)
     slot.unit_weights = f.kind != 'raw' and kind in ('single', 'seq', 'mseq')
     if f.kind == 'raw':
@@ -401,7 +440,9 @@ class InputLayer(object):
           if slot.bucket_mode == _lib.BUCKET_ONE_ROW and (uses[slot.table] > 1 or sc.kind != 'single'):
             slot.bucket_mode = _lib.BUCKET_NONE
     for a in self.arenas.values():
-      a.materialize(embedding_optimizer, generator=generator, adagrad_init=adagrad_init)
+      # a key-value table's rows are drawn when their key is first trained; the zero row stays zero
+      a.materialize(embedding_optimizer, generator=generator, adagrad_init=adagrad_init,
+                    init_fn=(lambda w: w.zero_()) if a.kv is not None else None)
       # tables of a backbone `embedding_layer` block: Keras Embedding's uniform(-limit, limit) initialiser
       for tname, limit in (uniform_tables or {}).items():
         if tname in a.tables and os.environ.get('ER_PLAN_ONLY') != '1':
@@ -418,8 +459,9 @@ class InputLayer(object):
     self._gather_plan = {}
     self.static_ids = {}
     self.static_w = {}
-    self.out_index = {}                        # (dim, out_key) -> (subcall key, local buf index)
-    for dim, subs in self.subcalls.items():
+    self.out_index = {}                        # (dim, out_key) -> (arena key, subcall key, local buf index)
+    for ak, subs in self.subcalls.items():
+      dim = self.arenas[ak].dim
       for sk, sc in subs.items():
         keys = list(dict.fromkeys(out_key for out_key, _, _, _ in sc.items))
         widths = [0] * len(keys)
@@ -431,33 +473,33 @@ class InputLayer(object):
         if sc.kind == 'tag':
           raw = sum(self.features[fn].raw_input_dim for _, fn, _, _ in sc.items if self.features[fn].kind == 'raw')
           cap = max_tag_lookups or 8 * B * len(slots) + B * raw
-          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=False, max_lookups=cap)
+          sc.call = E.ArenaCall(self.arenas[ak], slots, B, widths, single_valued=False, max_lookups=cap)
         elif sc.kind == 'mseq':
           cap = max_tag_lookups or 4 * B * sk[1] * len(slots)     # room for 4 values per step on average
-          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=False, max_lookups=cap)
+          sc.call = E.ArenaCall(self.arenas[ak], slots, B, widths, single_valued=False, max_lookups=cap)
         else:
-          sc.call = E.ArenaCall(self.arenas[dim], slots, B, widths, single_valued=True)
+          sc.call = E.ArenaCall(self.arenas[ak], slots, B, widths, single_valued=True)
         for j, k in enumerate(keys):
           # an output matrix belongs to one launch: lookup() finds each column's matrix by (dim, out_key)
           assert (dim, k) not in self.out_index, 'output %s of width %d written by two launches' % (k, dim)
-          self.out_index[(dim, k)] = (sk, j)
+          self.out_index[(dim, k)] = (ak, sk, j)
         if sc.kind == 'single':
-          self.calls[dim] = sc.call
+          self.calls[ak] = sc.call
           src = [s for _, _, _, s in sc.items]
-          self.static_ids[dim] = torch.zeros(sc.call.n_seg, dtype=torch.int64, device=device)
+          self.static_ids[ak] = torch.zeros(sc.call.n_seg, dtype=torch.int64, device=device)
           has_raw = any(k == 'raw' for k, _ in src)
-          self.static_w[dim] = (torch.ones(sc.call.n_seg, dtype=torch.float32, device=device)
-                                if has_raw else None)
+          self.static_w[ak] = (torch.ones(sc.call.n_seg, dtype=torch.float32, device=device)
+                               if has_raw else None)
           sc.call.identity_ids = ([k for k, _ in src] == ['id'] * len(src) and
                                   [i for _, i in src] == list(range(len(self.sparse_names))))
           sc.call.sources = src
-      self.merged[dim] = MergedCall(self.arenas[dim], list(subs.values()))
-    # every looked-up column reads its position from its own slot's ArenaCall
+      self.merged[ak] = MergedCall(self.arenas[ak], list(subs.values()))
+    # every looked-up column reads its position and its output matrix from its own slot's ArenaCall
     cols = {id(slot): c for subs in self.subcalls.values() for sc in subs.values()
             for slot, c in zip(sc.call.slots, sc.call.slot_cols)}
 
     def resolved(columns):
-      return [e if e.slot is None else e._replace(col=cols[id(e.slot)]) for e in columns]
+      return [e if e.slot is None else e._replace(col=cols[id(e.slot)], out_key=e.slot.out_key) for e in columns]
     self.group_layout = {g: resolved(lay) for g, lay in self.group_layout.items()}
     self.seq_layout = {s: dict(lay, key=resolved(lay['key']), hist=resolved(lay['hist']))
                        for s, lay in self.seq_layout.items()}
@@ -575,7 +617,8 @@ class InputLayer(object):
   def check_exchange(self):
     """EmbeddingParallel: raise if a per-peer block of the fixed-capacity exchange overflowed since the last check
     (reads one counter per arena back: call it outside the step loop, e.g. when the loss is logged), or if a prefetched
-    batch was not the one looked up.  Every exchange's counters are read and reset before the first error is raised."""
+    batch was not the one looked up.  Every exchange's counters are read and reset before the first error is raised.
+    Any run: then raise if a key-value table met more keys than its max_capacity (check_kv)."""
     err = None
     for ex in self._exchanges():
       ex.build()
@@ -583,8 +626,20 @@ class InputLayer(object):
         ex.check()
       except _lib.ErError as e:
         err = err or e
+    try:
+      self.check_kv()
+    except _lib.ErError as e:
+      err = err or e
     if err is not None:
       raise err
+
+  def check_kv(self):
+    """raise, naming the table and its max_capacity, if a key-value table met more distinct keys than it has rows
+    (reads two counters per table back: call it outside the step loop).  The lookups of the keys left without a row
+    were dropped."""
+    for a in self.arenas.values():
+      if a.kv is not None:
+        a.kv.check()
 
   def sparse_grad_sqnorm(self):
     """sum over the tables of ||IndexedSlices.values||^2 as TF would build them after loss.backward(): the gradient of a
@@ -641,6 +696,9 @@ class InputLayer(object):
     dense_norm = self.normalize_dense(dense) if dense is not None else None
     out = []
     self._preset_rows = {}
+    if any(a.kv is not None for a in self.arenas.values()):
+      raise NotImplementedError('ev_params (key-value tables) with tables replicated over data-parallel ranks: '
+                                'key-value tables train on one GPU')
     for dim, subs in self.subcalls.items():
       for sk, sc in subs.items():
         if sc.kind != 'single' or len(subs) != 1:
@@ -803,7 +861,8 @@ class InputLayer(object):
     return parts if prefetch else (parts, pool)
 
   def _run_subcall(self, dim, sk, sc, features, dense_norm):
-    """K1 + K2 of one uniform launch; returns (rows, weights, row_ptr, seg_ids, outs)."""
+    """K1 + K2 of one uniform launch of the arena keyed `dim` (its dim, or (dim, table) for a key-value table); returns
+    (rows, weights, row_ptr, seg_ids, outs)."""
     call = sc.call
     B = self.batch_size
     if self.ep and sc.kind != 'seq':
@@ -832,6 +891,11 @@ class InputLayer(object):
         self._rows_cache[key] = (rows, w)
       else:
         rows, w = hit
+      if call.arena.kv is not None:
+        buf = self._kv_bufs.get((dim, sk))
+        if buf is None:
+          buf = self._kv_bufs[(dim, sk)] = torch.empty_like(rows)   # (a stable address for graph capture)
+        rows = self._kv_rows(call.arena, rows, buf)
       outs = E.fused_lookup(call, rows, weights=w)
       return rows, w, None, None, outs
     if sc.kind == 'seq' and self.ep:
@@ -870,8 +934,21 @@ class InputLayer(object):
     rows = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
     K.bucketize(ids_cap, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr,
                 rows=rows, **K.k1_weight_args(ids_cap, weights))
+    rows = self._kv_rows(call.arena, rows, torch.empty_like(rows))
     outs = E.fused_lookup(call, rows, weights=weights, row_ptr=row_ptr)
     return rows, weights, row_ptr, seg_ids, outs
+
+  @staticmethod
+  def _kv_rows(arena, keys, out):
+    """a key-value table's lookups: the keys K1 wrote -> pool rows in `out`, inserting unseen keys when training (grad
+    enabled) and reading the zero row for them otherwise; other arenas' rows pass through"""
+    if arena.kv is None:
+      return keys
+    return arena.kv.lookup(keys, out, torch.is_grad_enabled())
+
+  def kv_sizes(self):
+    """{key-value table: keys that hold a row} (reads the device counters back)"""
+    return {a.kv.name: a.kv.size() for a in self.arenas.values() if a.kv is not None}
 
   def _csr_inputs(self, sc, features):
     """a multi-valued launch's ids padded to its lookup capacity, its lengths, and its weights (None: all 1)"""
@@ -957,15 +1034,15 @@ class InputLayer(object):
     self._ex_inputs = {}   # EmbeddingParallel: exchange -> its launches' pooling inputs, once it ran for this batch
     self._pending = []
     outs_by_key = {}
-    for dim, subs in self.subcalls.items():
+    for ak, subs in self.subcalls.items():
       parts = []
       for sk, sc in subs.items():
-        rows, w, row_ptr, seg_ids, outs = self._run_subcall(dim, sk, sc, features, dense_norm)
+        rows, w, row_ptr, seg_ids, outs = self._run_subcall(ak, sk, sc, features, dense_norm)
         parts.append((sc, rows, w, seg_ids, outs))
-        for (d, k), (skk, j) in self.out_index.items():
-          if d == dim and skk == sk:
-            outs_by_key[(dim, k)] = outs[j]
-      self._queue_update(self.merged[dim], parts)
+        for (d, k), (akk, skk, j) in self.out_index.items():
+          if akk == ak and skk == sk:
+            outs_by_key[(d, k)] = outs[j]
+      self._queue_update(self.merged[ak], parts)
     self._presort()
     self.seq_outputs = {}
     B = self.batch_size

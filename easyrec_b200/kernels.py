@@ -140,6 +140,46 @@ def bucketize_seq(ids, lens, batch, seq_len, slots_dev, n_slots, rows=None, owne
   return rows
 
 
+def kv_find_or_insert(index_keys, index_rows, capacity, stats, keys, rows, weight, state0, state1, state0_init, seed,
+                      init_stddev, init_truncated=True, shard_n=1, shard_rank=0):
+  """er_kv_find_or_insert: rows = the pool rows of the keys `keys * shard_n + shard_rank` (int64 keys from K1, -1
+  dropped); a key seen for the first time takes the next row, initialised from (seed, key) and the optimizer state's
+  initial values."""
+  for t, nm in ((index_keys, 'index_keys'), (index_rows, 'index_rows'), (stats, 'stats'), (keys, 'keys'), (rows, 'rows')):
+    _chk(t, torch.int64, nm)
+  assert rows.numel() == keys.numel() and index_rows.numel() == index_keys.numel()
+  _, stride = _chk_rows(weight, 'weight')
+  for st in (state0, state1):
+    if st is not None and _chk_rows(st, 'state')[1] != stride:
+      raise _lib.ErError('weight and optimizer state must share one row stride')
+  _lib.check(_lib.load().er_kv_find_or_insert(
+      _p(index_keys), _p(index_rows), index_keys.numel(), int(capacity), _p(stats), _p(keys), keys.numel(),
+      int(shard_n), int(shard_rank), _p(rows), _p(weight), _p(state0), _p(state1), stride, weight.shape[1],
+      float(state0_init), int(seed) & (2**64 - 1), float(init_stddev), int(bool(init_truncated)), _stream()),
+      'er_kv_find_or_insert')
+  return rows
+
+
+def kv_find(index_keys, index_rows, keys, zero_row, rows, shard_n=1, shard_rank=0):
+  """er_kv_find: rows = the pool rows of the keys `keys * shard_n + shard_rank`; keys without a row read `zero_row`,
+  nothing is inserted."""
+  for t, nm in ((index_keys, 'index_keys'), (index_rows, 'index_rows'), (keys, 'keys'), (rows, 'rows')):
+    _chk(t, torch.int64, nm)
+  assert rows.numel() == keys.numel()
+  _lib.check(_lib.load().er_kv_find(_p(index_keys), _p(index_rows), index_keys.numel(), _p(keys), keys.numel(),
+                                    int(shard_n), int(shard_rank), int(zero_row), _p(rows), _stream()), 'er_kv_find')
+  return rows
+
+
+def kv_insert_rows(index_keys, index_rows, keys, rows, stats):
+  """er_kv_insert_rows: put distinct `keys` into an empty index with the given pool `rows` (restore)."""
+  for t, nm in ((index_keys, 'index_keys'), (index_rows, 'index_rows'), (keys, 'keys'), (rows, 'rows'), (stats, 'stats')):
+    _chk(t, torch.int64, nm)
+  assert rows.numel() == keys.numel()
+  _lib.check(_lib.load().er_kv_insert_rows(_p(index_keys), _p(index_rows), index_keys.numel(), _p(keys), _p(rows),
+                                           keys.numel(), _p(stats), _stream()), 'er_kv_insert_rows')
+
+
 def k1_weight_args(ids, weights):
   """Keyword arguments of bucketize() that hand a weighted CSR call's lookup weights to K1, so that the lookups the
   pooling prunes are dropped before K7, er_mark_rows and K8 see them.  Only device tensors take this path: the host

@@ -192,6 +192,11 @@ class ShardedExchange(object):
       K.shard_group(self.rows_local, self.owner, N, self.cap, self.send_rows, self.pos, self.counts, self.group_ws)
       self.overflow += self.counts[N:]
       dist.all_to_all_single(self.recv_rows, self.send_rows)
+    # key-value tables (ev_params): the owner turns the keys it received (key div N) into rows of its pool, inserting
+    # unseen keys when training; the requester side and the prefetched id half never see a row number
+    for h in self.heads:
+      if h.call.arena.kv is not None:
+        h.call.arena.kv.lookup(self.recv_rows, h.owner_rows, torch.is_grad_enabled())
     self.placements.clear()
     if self._side is not None and torch.is_grad_enabled():
       # the row-only halves of the K7s (requester: positions of the single-valued launches, owner: received rows)
@@ -204,9 +209,9 @@ class ShardedExchange(object):
           if not m.csr:
             self.placements.presort(m.pos, self.n_ex, a.dim, m.pool_ws, m.pool_slots, m.call.n_slots)
           if m.head is m:
-            self.placements.presort(self.recv_rows, a.n_rows, a.dim, m.owner_ws, m.owner_slots, 1)
+            self.placements.presort(m.owner_rows, a.n_rows, a.dim, m.owner_ws, m.owner_slots, 1)
     for h in self.heads:
-      K.embedding_fwd(h.call.arena.weight, h.call.arena.dim, self.recv_rows, h.owner_slots, 1, self.n_ex, [self.send_emb])
+      K.embedding_fwd(h.call.arena.weight, h.call.arena.dim, h.owner_rows, h.owner_slots, 1, self.n_ex, [self.send_emb])
     dist.all_to_all_single(self.recv_emb, self.send_emb)
     self._active, self._summed = [], 0
 
@@ -220,10 +225,10 @@ class ShardedExchange(object):
       opt.grad_scale = opt.grad_scale / N
     for h in dict.fromkeys(m.head for m in self._active):
       a = h.call.arena
-      K.embedding_bwd(a.weight, a.state0, a.state1, a.dim, self.recv_rows, h.owner_slots, 1, self.n_ex, [self.recv_g],
+      K.embedding_bwd(a.weight, a.state0, a.state1, a.dim, h.owner_rows, h.owner_slots, 1, self.n_ex, [self.recv_g],
                       opt, h.owner_ws, n_rows=a.n_rows,
-                      sorted_from=self.placements.sorted_from(self.recv_rows, a.n_rows, a.dim, h.owner_ws))
-      E.adam_dense_decay(a, self.recv_rows, opt)
+                      sorted_from=self.placements.sorted_from(h.owner_rows, a.n_rows, a.dim, h.owner_ws))
+      E.adam_dense_decay(a, h.owner_rows, opt)
     if struct_scaled:
       opt.grad_scale = opt.grad_scale * N
     self._active, self._summed = [], 0
@@ -310,6 +315,8 @@ class ShardedLookup(object):
                   shard_n=1)]
       self.owner_slots = K.slots_to_device(K.make_slots(own, D), dev)
       self.owner_ws = K.bwd_workspace(ex.n_ex, dev, D)
+      # the arena rows of the received ids: the ids themselves, or a key-value table's pool rows for the keys
+      self.owner_rows = (torch.empty(ex.n_ex, dtype=torch.int64, device=dev) if a.kv is not None else ex.recv_rows)
     self.pool_ws = K.bwd_workspace(self.L, dev, D)
     self.recv_view = ex.recv_emb[:, self.col:self.col + D]   # this arena's received rows: the pooling K2's "table"
     self.sum_view = ex.send_g[:, self.col:self.col + D]      # ... and the requester-side gradient sums

@@ -234,12 +234,14 @@ def write_c2_binary(prefix, n_batches, batch_size, n_files, seed=20240, uniform=
 
 
 def c4_config_text(batch_size=4096, item_vocab=200_000_000, user_vocab=10_000_000, emb_dim=16, lr=0.01,
-                   embedding_parallel=True):
+                   embedding_parallel=True, kv_capacity=0):
   """C4 of BASELINE.json as a pipeline config: DSSM two towers (samples/model_config/dssm_on_taobao.config's shape:
   user side = user id + 4 profile ids, item side = item id + category + brand + price), cosine similarity with
   in-batch negatives (loss_type SOFTMAX_CROSS_ENTROPY, model/dssm.py + match_model.py:95-165), the item table
-  row-sharded (train_distribute: EmbeddingParallelStrategy)."""
-  return ('''
+  row-sharded (train_distribute: EmbeddingParallelStrategy).  kv_capacity > 0: user_id and item_id are key-value
+  tables (ev_params { max_capacity: kv_capacity }) instead of hash_bucket_size-row tables."""
+  ev = ' ev_params { max_capacity: %d }' % kv_capacity if kv_capacity else ''
+  text = ('''
 train_config { log_step_count_steps: 1000000 %s
   optimizer_config { adagrad_optimizer { learning_rate { constant_learning_rate { learning_rate: %g } } } } }
 data_config { batch_size: %d input_type: DummyInput label_fields: "clk"
@@ -249,12 +251,12 @@ data_config { batch_size: %d input_type: DummyInput label_fields: "clk"
   input_fields { input_name: "item_id" input_type: INT64 } input_fields { input_name: "cate_id" input_type: INT64 }
   input_fields { input_name: "brand" input_type: INT64 } input_fields { input_name: "price" input_type: FLOAT } }
 feature_config {
-  features { input_names: "user_id" feature_type: IdFeature embedding_dim: %d hash_bucket_size: %d }
+  features { input_names: "user_id" feature_type: IdFeature embedding_dim: %d hash_bucket_size: %d EV }
   features { input_names: "age" feature_type: IdFeature embedding_dim: %d num_buckets: 100 }
   features { input_names: "gender" feature_type: IdFeature embedding_dim: %d num_buckets: 3 }
   features { input_names: "city" feature_type: IdFeature embedding_dim: %d hash_bucket_size: 10000 }
   features { input_names: "level" feature_type: IdFeature embedding_dim: %d num_buckets: 10 }
-  features { input_names: "item_id" feature_type: IdFeature embedding_dim: %d hash_bucket_size: %d }
+  features { input_names: "item_id" feature_type: IdFeature embedding_dim: %d hash_bucket_size: %d EV }
   features { input_names: "cate_id" feature_type: IdFeature embedding_dim: %d hash_bucket_size: 10000 }
   features { input_names: "brand" feature_type: IdFeature embedding_dim: %d hash_bucket_size: 1000000 }
   features { input_names: "price" feature_type: RawFeature embedding_dim: %d min_val: 0.0 max_val: 1.0 } }
@@ -266,7 +268,8 @@ model_config { model_class: "DSSM"
          simi_func: COSINE temperature: 0.05 scale_simi: true l2_regularization: 1e-6 }
   loss_type: SOFTMAX_CROSS_ENTROPY embedding_regularization: 5e-5 }
 ''' % ('train_distribute: EmbeddingParallelStrategy' if embedding_parallel else '', lr, batch_size,
-       emb_dim, user_vocab, emb_dim, emb_dim, emb_dim, emb_dim, emb_dim, item_vocab, emb_dim, emb_dim, emb_dim)).encode()
+       emb_dim, user_vocab, emb_dim, emb_dim, emb_dim, emb_dim, emb_dim, item_vocab, emb_dim, emb_dim, emb_dim))
+  return text.replace(' EV }', ev + ' }').encode()
 
 
 def c4_batch(batch_size, seed, zipf_alpha=1.05):

@@ -715,6 +715,40 @@ int er_binary_unpack(const int32_t* label, const float* dense, const uint32_t* c
 int er_load_embed(const char* ckpt_path, const char* var_name, int32_t task_index, int32_t task_num,
                   int32_t embed_dim, int64_t embed_part_size, float* vals, int64_t* rows_loaded);
 
+/* ---- key-value embedding tables (ev_params; feature_column/feature_column.py:250-256,288-291, SOK DynamicVariable at
+ * compat/feature_column/feature_column.py:425-503) ----
+ * A KV table's slots have num_buckets = 2^63 - 1, so K1 writes the KEY (>= 0, or -1 for a dropped lookup) where a
+ * static table has its row.  These calls turn keys into rows of a pool of `capacity` rows through an open-addressing
+ * index: index_keys int64[n_index] (every entry ER_KV_EMPTY before first use) and index_rows int64[n_index], n_index a
+ * power of two >= 16 and >= 2 * capacity.  stats int64[2]: [0] rows handed out so far (may pass capacity: the keys
+ * beyond it have no row), [1] live lookups that were left without a row.  The host reads stats outside the step.
+ * Row numbers depend on the order of claims and are not deterministic; nothing else does.  No allocation, no host
+ * synchronisation, and no thread waits on another thread's store. */
+#define ER_KV_EMPTY (-1)
+
+/* Training lookup: find-or-insert.  The key of lookup l is keys[l] * shard_n + shard_rank (keys[l] < 0: none): a
+ * row-sharded table's owner passes the owner-local keys it received (K1's key div N) and its rank, an unsharded table
+ * 1 and 0.  rows[l] = the pool row of that key (-1 without a key or when the pool has no row left for it).  A key seen
+ * for the first time is claimed in the index and, while the pool has rows, gets the next one, initialised: weight[row,
+ * c] = a normal(0, init_stddev), truncated at 2 init_stddev when init_truncated, drawn from a counter-based hash of
+ * (seed, key, c); state0 (may be null) = state0_init and state1 (may be null) = 0 over the row's dim columns.  weight /
+ * state0 / state1 share row_stride (floats).  Two launches: claim and initialise, then resolve.  keys and rows must
+ * not alias. */
+int er_kv_find_or_insert(int64_t* index_keys, int64_t* index_rows, int64_t n_index, int64_t capacity,
+                         int64_t* stats, const int64_t* keys, int64_t n, int32_t shard_n, int32_t shard_rank,
+                         int64_t* rows, float* weight, float* state0, float* state1, int64_t row_stride, int32_t dim,
+                         float state0_init, uint64_t seed, float init_stddev, int32_t init_truncated,
+                         er_stream_t stream);
+/* Evaluation / prediction lookup: find only, keys as in er_kv_find_or_insert.  rows[l] = the row of the key; a key
+ * without a row reads zero_row (a row the caller keeps at zero: "new key will get zero embedding",
+ * feature_column_v2.py:3489-3494); keys[l] < 0 -> -1. */
+int er_kv_find(const int64_t* index_keys, const int64_t* index_rows, int64_t n_index, const int64_t* keys,
+               int64_t n, int32_t shard_n, int32_t shard_rank, int64_t zero_row, int64_t* rows, er_stream_t stream);
+/* Restore: insert keys[i] with the given row rows[i], for distinct keys >= 0 into an empty index (2 * n <= n_index).  A
+ * negative or repeated key counts in stats[1]; stats[0] is the caller's to set. */
+int er_kv_insert_rows(int64_t* index_keys, int64_t* index_rows, int64_t n_index, const int64_t* keys,
+                      const int64_t* rows, int64_t n, int64_t* stats, er_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
