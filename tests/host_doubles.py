@@ -157,7 +157,7 @@ def install_sparse(patch):
     cnt = np.zeros(world + 1, np.int32)
     seen = {}
     for l in range(r.size):
-      if r[l] < 0 or o[l] < 0:
+      if r[l] < 0 or o[l] < 0 or o[l] >= world:   # (an owner outside [0, world) is not counted, as in the kernel)
         continue
       key = (int(o[l]), int(r[l]))
       if key not in seen:

@@ -74,12 +74,14 @@ def kv_rows(il):
   return out
 
 
-def _worker(rank, port, ret, world, tmp):
+def _worker(rank, port, ret, world, tmp, cuda=False):
+  """cuda: NCCL and the real kernels on cuda:rank (tests/test_gpu_dp_extra.py); else gloo and the kernel doubles"""
   sys.path.insert(0, HERE)
   from test_dp_clip_gloo import _setup
-  dev = _setup(rank, port, world, False)
-  import kv_doubles
-  kv_doubles.install()
+  dev = _setup(rank, port, world, cuda)
+  if not cuda:
+    import kv_doubles
+    kv_doubles.install()
   from easyrec_b200 import checkpoint
   from easyrec_b200.estimator import EasyRecEstimator
   ep = EasyRecEstimator(CFG, device=dev, seed=5, world_size=world, rank=rank, embedding_parallel=None)
@@ -98,11 +100,11 @@ def _worker(rank, port, ret, world, tmp):
   ep.trainer.dense_opt.flat_p.copy_(ref.trainer.dense_opt.flat_p)
   for step in range(4):
     ids, tags, lens, labels = batch(rank, step)
-    l_ep, p_ep = ep.trainer.train_step(feats(ids, tags, lens, dev), torch.from_numpy(labels))
+    l_ep, p_ep = ep.trainer.train_step(feats(ids, tags, lens, dev), torch.from_numpy(labels).to(dev))
     cids, ctags, clens, clabels = concatenated(world, step)
-    l_ref, p_ref = ref.trainer.train_step(feats(cids, ctags, clens, dev), torch.from_numpy(clabels))
+    l_ref, p_ref = ref.trainer.train_step(feats(cids, ctags, clens, dev), torch.from_numpy(clabels).to(dev))
     assert float((p_ep - p_ref[rank * B:(rank + 1) * B]).abs().max()) < 1e-5, (step, p_ep, p_ref)
-    mean = torch.tensor([float(l_ep)])
+    mean = torch.tensor([float(l_ep)], device=dev)
     dist.all_reduce(mean)
     assert abs(float(mean) / world - float(l_ref)) < 1e-5, (step, float(mean) / world, float(l_ref))
   ep.input_layer.check_exchange()

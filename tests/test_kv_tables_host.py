@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 import torch
 
-from easyrec_b200 import _lib, builder, checkpoint, embedding as E, input_layer as IL
+from easyrec_b200 import _lib, builder, checkpoint, embedding as E, input_layer as IL, kernels as K
 from easyrec_b200.config import config_util
 
 import host_doubles  # noqa: E402  (tests/ is on sys.path under pytest's rootdir conftest)
@@ -90,18 +90,25 @@ def per_key(il, table):
   return out
 
 
-def restate(steps, kind, lr=0.05, b1=0.9, b2=0.999, eps=1e-8, acc0=0.1):
-  """float64: {table: {key: [w, s0, s1]}} after `steps` [(batch, R)]"""
-  ref = {'item_embedding': {}, 'tags_embedding': {}}
-  std = 0.01 / math.sqrt(DIM)
+def restate(steps, kind, lr=0.05, b1=0.9, b2=0.999, eps=1e-8, acc0=0.1, grads_of=key_grads):
+  """float64: {table: {key: [w, s0, s1]}} after `steps` [(batch, R)].  kind: 'sgd', 'adagrad', 'momentum' (momentum b1)
+  or 'adam' / 'lazy_adam' (both the touched-row rule on a key-value table).  grads_of(batch, R) -> {table: {key: summed
+  gradient}}: every key a step looked up, a zero gradient included"""
+  ref = {}
   for t, (batch, R) in enumerate(steps):
-    for table, grads in key_grads(batch, R).items():
+    for table, grads in grads_of(batch, R).items():
       for k, g in grads.items():
-        if k not in ref[table]:
-          w0 = kv_doubles.init_values(table_seed(table), [k], DIM, std)[0].astype(np.float64)
-          ref[table][k] = [w0, np.full(DIM, acc0 if kind == 'adagrad' else 0.0), np.zeros(DIM)]
+        if k not in ref.setdefault(table, {}):
+          dim = g.size
+          w0 = kv_doubles.init_values(table_seed(table), [k], dim, 0.01 / math.sqrt(dim))[0].astype(np.float64)
+          ref[table][k] = [w0, np.full(dim, acc0 if kind == 'adagrad' else 0.0), np.zeros(dim)]
         w, s0, s1 = ref[table][k]
-        if kind == 'adagrad':
+        if kind == 'sgd':
+          w = w - lr * g
+        elif kind == 'momentum':
+          s0 = b1 * s0 + g
+          w = w - lr * s0
+        elif kind == 'adagrad':
           s0 = s0 + g * g
           w = w - lr * g / np.sqrt(s0)
         else:
@@ -114,31 +121,17 @@ def restate(steps, kind, lr=0.05, b1=0.9, b2=0.999, eps=1e-8, acc0=0.1):
 
 
 @pytest.mark.parametrize('kind,opt', [('adagrad', _lib.OPT_ADAGRAD), ('lazy_adam', _lib.OPT_LAZY_ADAM),
-                                      ('adam', _lib.OPT_ADAM_ROWS)])
+                                      ('adam', _lib.OPT_ADAM_ROWS), ('sgd', _lib.OPT_SGD),
+                                      ('momentum', _lib.OPT_MOMENTUM)])
 def test_three_steps_match_a_float64_restatement_per_key(doubles, kind, opt):
-  il = make_layer(opt)
-  rng = np.random.default_rng(3)
-  steps = []
-  for t in range(3):
-    feats, batch = make_batch(rng)
-    R = torch.tensor(rng.integers(-3, 4, (B, 3 * DIM)) / 4.0, dtype=torch.float32)
-    steps.append((batch, R))
-    train_step(il, feats, R, 0.05, t)
-  ref = restate(steps, 'adagrad' if kind == 'adagrad' else 'adam')
-  for table in ref:
-    got = per_key(il, table)
-    assert set(got) == set(ref[table])
-    assert il.kv_sizes()[table] == len(ref[table])
-    for k, (w, s0, s1) in ref[table].items():
-      gw, g0, g1 = got[k]
-      np.testing.assert_allclose(gw, w, atol=1e-6, rtol=0, err_msg='%s key %d' % (table, k))
-      np.testing.assert_allclose(g0, s0, atol=1e-6, rtol=0)
-      if kind != 'adagrad':
-        np.testing.assert_allclose(g1, s1, atol=1e-6, rtol=0)
+  import test_gpu_kv_f64 as G
+  il, steps = G.train_model(opt, 'cpu', prune=False)
+  ref = restate(steps, kind, grads_of=G.model_grads)
+  G.check_per_key(il, ref, kind, 1e-6)
   if kind == 'adam':
     # adam_optimizer on a key-value table is the touched-row rule: no dense sweep, keys a step did not see stay put
     assert il.arenas[(DIM, 'item_embedding')].touched is None
-    untouched = set(ref['item_embedding']) - set(key_grads(steps[-1][0], steps[-1][1])['item_embedding'])
+    untouched = set(ref['item_embedding']) - set(G.model_grads(*steps[-1])['item_embedding'])
     assert untouched, 'the batches should leave some item key out of the last step'
 
 
@@ -345,3 +338,56 @@ def test_a_table_shared_by_static_and_key_value_features_is_refused():
            IL.id_feature('b', DIM, hash_bucket_size=50, embedding_name='t', kv_capacity=10)]
   with pytest.raises(ValueError, match='table t: read by features with different ev_params'):
     IL.InputLayer(feats, collections.OrderedDict(g=dict(features=['a', 'b'])), B, 'cpu')
+
+
+# ---- the restatements of test_gpu_kv_f64 against the doubles --------------------------------------------------------------
+@pytest.mark.parametrize('shard_n', [1, 3, 100])
+@pytest.mark.parametrize('mode', [_lib.BUCKET_FARM_DECIMAL, _lib.BUCKET_MOD, _lib.BUCKET_IDENTITY])
+def test_k1_kv_restatement_on_the_host_doubles(doubles, mode, shard_n):
+  import test_gpu_kv_f64 as G
+  ids = G.kv_edge_ids(np.random.default_rng(mode), 50)
+  sl = G._k1_slots(mode, shard_n, ids.size, 0)[:1]      # one summed slot, a lookup per segment
+  rows, owner = torch.empty(ids.size, dtype=torch.int64), torch.empty(ids.size, dtype=torch.int32)
+  K.bucketize(torch.from_numpy(ids), K.slots_to_device(sl, 'cpu'), 1, ids.size, rows=rows, owner=owner)
+  assert (rows.tolist(), owner.tolist()) == G.k1_kv_ref(ids, mode, shard_n)
+
+
+@pytest.mark.parametrize('world,n', [(1, 31), (3, 257), (65, 257), (200, 31)])
+def test_k8_checker_on_the_host_double(doubles, world, n):
+  import test_gpu_kv_f64 as G
+  rows, owner = G.k8_case(world, n, world + n)
+  live = (rows >= 0) & (owner >= 0) & (owner < world)
+  mx = int(np.bincount(np.unique(np.stack([rows[live], owner[live]], 1), axis=0)[:, 1], minlength=world).max())
+  for cap in (mx - 1, mx):
+    send, pos = torch.empty(world * cap, dtype=torch.int64), torch.empty(n, dtype=torch.int64)
+    counts = torch.empty(world + 1, dtype=torch.int32)
+    K.shard_group(torch.from_numpy(rows), torch.from_numpy(owner.astype(np.int32)), world, cap, send, pos, counts,
+                    K.shard_group_workspace(n, 'cpu'))
+    G.k8_check(rows, owner, world, cap, send.numpy(), pos.numpy(), counts.numpy())
+  # and it refuses the old packing's answer: two pairs that pack to one integer under owner << 48 | row share a position
+  if world >= 2:
+    p = pos.numpy().copy()
+    p[1], p[2] = p[0], p[0]      # k8_case puts (5 + 2^48, 0) at 0 and 1, (5, 1) at 2 and 3
+    with pytest.raises(AssertionError):
+      G.k8_check(rows, owner, world, mx, send.numpy(), p, counts.numpy())
+
+
+def test_index_model_on_the_kv_doubles(doubles):
+  import test_gpu_kv_f64 as G
+  rng = np.random.default_rng(4)
+  capacity, n_index = 40, 128
+  keys = rng.permutation(np.concatenate([rng.integers(0, 2 ** 63 - 1, 50, dtype=np.int64)] * 2 + [[-1]])).tolist()
+  ik, ir = torch.full((n_index,), _lib.KV_EMPTY, dtype=torch.int64), torch.full((n_index,), -1, dtype=torch.int64)
+  stats = torch.zeros(2, dtype=torch.int64)
+  rows = torch.empty(len(keys), dtype=torch.int64)
+  w = torch.zeros(capacity + 1, DIM)
+  K.kv_find_or_insert(ik, ir, capacity, stats, torch.tensor(keys), rows, w, None, None, 0.0, 5, 0.01)
+  held = G.index_check(keys, rows.tolist(), ik, ir, stats, capacity, n_index)
+  assert len(held) == 50 and stats.tolist() == [50, sum(1 for k, r in zip(keys, rows.tolist()) if k >= 0 and r < 0)]
+
+
+@pytest.mark.parametrize('kv', [True, False], ids=['key_value', 'static'])
+def test_sparse_norm_restatement_on_the_host_doubles(doubles, kv):
+  import test_gpu_kv_f64 as G
+  for got, want in G.norm_steps(kv, 'cpu'):
+    assert abs(got - want) <= 1e-5 * want
