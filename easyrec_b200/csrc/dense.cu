@@ -576,11 +576,11 @@ __device__ __forceinline__ uint32_t drop_bits(uint64_t seed, uint64_t ctr, uint6
 }
 
 __global__ void __launch_bounds__(256)
-    dropout_kernel(const float* __restrict__ x, int64_t n, uint32_t keep_thresh, float inv_keep, uint64_t seed,
+    dropout_kernel(const float* __restrict__ x, int64_t n, uint64_t keep_thresh, float inv_keep, uint64_t seed,
                    const int64_t* __restrict__ counter, float* __restrict__ y) {
   const uint64_t ctr = (uint64_t)*counter;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    y[i] = drop_bits(seed, ctr, (uint64_t)i) < keep_thresh ? x[i] * inv_keep : 0.f;
+    y[i] = (uint64_t)drop_bits(seed, ctr, (uint64_t)i) < keep_thresh ? x[i] * inv_keep : 0.f;
 }
 }  // namespace er
 
@@ -589,8 +589,10 @@ extern "C" int er_dropout(const float* x, int64_t n, float rate, uint64_t seed, 
   using namespace er;
   ER_REQUIRE(x && y && counter_dev, "null argument");
   ER_REQUIRE(n > 0 && rate >= 0.f && rate < 1.f, "rate must be in [0, 1)");
+  // kept iff the 32-bit draw is below floor(keep * 2^32), compared in 64 bits: at rate 0 the threshold is 2^32 and
+  // every draw, 0xffffffff included, keeps its element
   const double keep = 1.0 - (double)rate;
-  const uint32_t thresh = keep >= 1.0 ? 0xffffffffu : (uint32_t)(keep * 4294967296.0);
+  const uint64_t thresh = (uint64_t)(keep * 4294967296.0);
   dropout_kernel<<<grid_for(n, 256, 8), 256, 0, as_stream(stream)>>>(x, n, thresh, (float)(1.0 / keep), seed, counter_dev, y);
   count_launches(1);
   ER_CUDA_LAUNCH_CHECK();

@@ -37,7 +37,10 @@ ER_HD float act_slope(float x) {
   if (KIND == ER_ACT_GELU) {
     const float c = 0.7978845608028654f;
     const float t = tanhf(c * (x + 0.044715f * (x * x * x)));
-    return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * c * (1.0f + 3.0f * 0.044715f * x * x);
+    const float sech2 = 1.0f - t * t;
+    // once tanh saturates the second term is 0 (0 * x keeps its sign, and NaN at x = +-inf); without the branch
+    // 1 + 0.134 x^2 overflows for |x| > 5e19 and the product 0 * inf turns a slope of 1 or 0 into NaN
+    return 0.5f * (1.0f + t) + (sech2 == 0.f ? 0.f * x : 0.5f * x * sech2 * c * (1.0f + 3.0f * 0.044715f * x * x));
   }
   if (KIND == ER_ACT_LEAKY_RELU) return x > 0.f ? 1.0f : 0.2f;
   if (KIND == ER_ACT_ELU) return x < 0.f ? expf(x) : 1.0f;

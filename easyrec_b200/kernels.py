@@ -222,10 +222,22 @@ def act_bwd(x, gy, kind):
   return gx
 
 
+def _chk_dice(x, alpha, **same):
+  """x [batch, units]; every tensor in `same` the same shape as x; alpha [units]"""
+  if x.dim() != 2:
+    raise _lib.ErError('x must be [batch, units], got %s' % (tuple(x.shape),))
+  for nm, t in same.items():
+    if t.shape != x.shape:
+      raise _lib.ErError('%s must have the shape of x %s, got %s' % (nm, tuple(x.shape), tuple(t.shape)))
+  if alpha.dim() != 1 or alpha.numel() != x.shape[1]:
+    raise _lib.ErError('alpha must be [%d], got %s' % (x.shape[1], tuple(alpha.shape)))
+
+
 def dice_fwd(x, xn, alpha):
   """er_dice_fwd: alpha * (1 - sigmoid(xn)) * x + sigmoid(xn) * x over [batch, units]."""
   for t, nm in ((x, 'x'), (xn, 'xn'), (alpha, 'alpha')):
     _chk(t, torch.float32, nm)
+  _chk_dice(x, alpha, xn=xn)
   y = torch.empty_like(x)
   _lib.check(_lib.load().er_dice_fwd(_p(x), _p(xn), _p(alpha), x.shape[0], x.shape[1], _p(y), _stream()), 'er_dice_fwd')
   return y
@@ -236,6 +248,7 @@ def dice_bwd(x, xn, alpha, gy):
   gy = gy.contiguous()
   for t, nm in ((x, 'x'), (xn, 'xn'), (alpha, 'alpha'), (gy, 'gy')):
     _chk(t, torch.float32, nm)
+  _chk_dice(x, alpha, xn=xn, gy=gy)
   gd, gn, ga = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
   _lib.check(_lib.load().er_dice_bwd(_p(x), _p(xn), _p(alpha), _p(gy), x.shape[0], x.shape[1], _p(gd), _p(gn), _p(ga),
                                      _stream()), 'er_dice_bwd')

@@ -406,8 +406,11 @@ int er_bias_bn_act_bwd(const float* z, const float* bias, const float* gamma,
                        float* gbeta, void* ws, size_t ws_bytes, er_stream_t stream);
 
 /* tf.nn.dropout of DNN.__call__ (layers/dnn.py:77-82): y = x * mask / (1 - rate), mask ~ Bernoulli(1 - rate) per
- * element, a counter-based function of (seed, *counter_dev, element index).  The backward pass is the SAME call on the
- * upstream gradient (same seed, same counter value): the mask is recomputed, not stored.  counter_dev is a device
+ * element, a counter-based function of (seed, *counter_dev, element index): element i is kept iff the top 32 bits of
+ * the splitmix64 finaliser of seed + counter * 0x9E3779B97F4A7C15 + i * 0xD1B54A32D192ED03 are below
+ * floor((1 - rate) * 2^32), so rate 0 keeps every element; a kept value is x * fp32(1 / (1 - rate)).  The backward
+ * pass is the SAME call on the upstream gradient (same seed, same counter value): the mask is recomputed, not stored.
+ * counter_dev is a device
  * int64 the caller advances once per step, so a captured graph draws a new mask on every replay. */
 int er_dropout(const float* x, int64_t n, float rate, uint64_t seed, const int64_t* counter_dev, float* y,
                er_stream_t stream);
