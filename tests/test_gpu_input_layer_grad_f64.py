@@ -286,16 +286,17 @@ class Reference(object):
     if combiner != 'sum':
       keep &= (wt.numpy() > 0)
     rows = np.where(keep, rows, -1)
+    # a pruned lookup contributes nothing, whatever its weight (a NaN weight of a mean / sqrtn lookup is pruned)
+    wt = torch.where(torch.from_numpy(keep), wt, torch.zeros_like(wt))
     e = self.gather(tname, dim, rows) * wt[:, None]
-    kt = torch.from_numpy(keep).to(self.dt)
     segt = torch.from_numpy(seg)
     out = torch.zeros(lens.size, dim, dtype=self.dt).index_add(0, segt, e)
     if combiner == 'sum':
       return out
     if combiner == 'mean':
-      d = torch.zeros(lens.size, dtype=self.dt).index_add(0, segt, wt * kt)
+      d = torch.zeros(lens.size, dtype=self.dt).index_add(0, segt, wt)
     else:
-      d = torch.sqrt(torch.zeros(lens.size, dtype=self.dt).index_add(0, segt, wt * wt * kt))
+      d = torch.sqrt(torch.zeros(lens.size, dtype=self.dt).index_add(0, segt, wt * wt))
     return torch.where(d[:, None] != 0, out / torch.where(d != 0, d, torch.ones_like(d))[:, None], torch.zeros_like(out))
 
   def lookup(self, name, tname, dim, wide=False):
