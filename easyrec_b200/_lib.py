@@ -28,7 +28,10 @@ assert SLOT_DTYPE.itemsize == 48
 DENSE_SEG_DTYPE = np.dtype([('offset', '<i8'), ('n', '<i8'), ('l2', '<f4'), ('lr_mult', '<f4')], align=True)
 assert DENSE_SEG_DTYPE.itemsize == 24
 
-BUCKET_FARM_DECIMAL, BUCKET_MOD, BUCKET_IDENTITY, BUCKET_NONE, BUCKET_ONE_ROW = 0, 1, 2, 3, 4
+BUCKET_FARM_DECIMAL, BUCKET_MOD, BUCKET_IDENTITY, BUCKET_NONE, BUCKET_ONE_ROW, BUCKET_VOCAB = 0, 1, 2, 3, 4, 5
+# er_vocab_t, 24 bytes: a vocabulary's index (device pointers) for the ER_BUCKET_VOCAB slots of a K1 call
+VOCAB_DTYPE = np.dtype([('index_keys', '<u8'), ('index_rows', '<u8'), ('n_index', '<i8')], align=True)
+assert VOCAB_DTYPE.itemsize == 24
 COMBINER_SUM, COMBINER_MEAN, COMBINER_SQRTN = 0, 1, 2
 COMBINER_UNIT_WEIGHTS = 16   # flag OR-ed into er_slot_t.combiner: the slot's weights[] entries are all 1.0
 OPT_SGD, OPT_ADAGRAD, OPT_LAZY_ADAM, OPT_ADAM_ROWS, OPT_MOMENTUM = 0, 1, 2, 3, 4
@@ -86,6 +89,8 @@ SIGNATURES = {
     'er_bucketize_weighted': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i32,
                                       c_vp, c_vp, c_vp]),
     'er_bucketize_seq': (c_i32, [c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp]),
+    'er_bucketize_vocab': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
+    'er_bucketize_seq_vocab': (c_i32, [c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'er_dropout': (c_i32, [c_vp, c_i64, ctypes.c_float, ctypes.c_uint64, c_vp, c_vp, c_vp]),
     'er_gemm_small_workspace_bytes': (c_sz, [c_i64, c_i64, c_i64]),
     'er_gemm_small': (c_i32, [c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_sz,

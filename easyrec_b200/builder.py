@@ -23,6 +23,74 @@ def ev_params(pipeline_config, fc):
   return mc.ev_params if mc.HasField('ev_params') else None
 
 
+def vocab_entries(fc):
+  """The vocabulary of a feature as a list of byte strings, or None.  The rule is picked in the reference's order,
+  hash_bucket_size, then vocab_list, then vocab_file (feature_column/feature_column.py:270-294); vocab_file holds one
+  entry per line, keyed on the whole line, and its size is the file's line count (:243-249), a last line without
+  '\n' included."""
+  if fc.hash_bucket_size > 0:
+    return None
+  if len(fc.vocab_list) > 0:
+    return [v.encode('utf-8') for v in fc.vocab_list]
+  if fc.HasField('vocab_file'):
+    with open(fc.vocab_file, 'rb') as f:
+      lines = f.read().split(b'\n')
+    if lines[-1] == b'':
+      lines.pop()        # the newline that ends the last line starts no entry
+    return lines
+  return None
+
+
+def vocab_keys(name, entries):
+  """Entry i of a vocabulary -> its 63-bit key Fingerprint64(entry) % (2^63 - 1), the key the readers give the
+  feature's raw strings; K1 reads row i for it.  Repeated entries are refused as TF's vocabulary tables refuse them, and
+  two entries whose keys collide are refused because K1 could not tell them apart."""
+  if not entries:
+    raise ValueError('feature %s: the vocabulary is empty' % name)
+  shown = lambda e: e.decode('utf-8', 'replace')   # noqa: E731
+  repeated = [shown(e) for e, c in collections.Counter(entries).items() if c > 1]
+  if repeated:
+    raise ValueError('feature %s: vocabulary entries %s appear more than once (a vocabulary table keys each entry '
+                     'once)' % (name, repeated[:10]))
+  keys = [_lib.fingerprint64(e) % _lib.KV_BUCKETS for e in entries]
+  first = {}
+  for e, k in zip(entries, keys):
+    if k in first:
+      raise NotImplementedError('feature %s: vocabulary entries %r and %r have the same 63-bit key %d '
+                                '(Fingerprint64 %% (2^63 - 1)); K1 cannot tell them apart' % (name, shown(first[k]),
+                                                                                          shown(e), k))
+    first[k] = e
+  return tuple(keys)
+
+
+def vocabulary(pipeline_config, fc, name, field_types, kv):
+  """The keys of a feature's vocabulary (vocab_keys) or None; refuses by name what cannot take one"""
+  if fc.hash_bucket_size > 0 and (len(fc.vocab_list) > 0 or fc.HasField('vocab_file')):
+    raise NotImplementedError('feature %s: hash_bucket_size together with vocab_list / vocab_file: the reference '
+                              'hashes and never reads the vocabulary (feature_column/feature_column.py:270-294); keep '
+                              'one of them' % name)
+  entries = vocab_entries(fc)
+  if entries is None:
+    return None
+  ftype = ftype_name(fc)
+  if ftype not in ('IdFeature', 'TagFeature', 'SequenceFeature'):
+    raise NotImplementedError('feature %s: vocab_list / vocab_file on a %s; vocabularies are read by IdFeatures, '
+                              'TagFeatures and SequenceFeatures' % (name, ftype))
+  if kv:
+    raise NotImplementedError('feature %s: vocab_list / vocab_file together with ev_params: a vocabulary column has '
+                              'a fixed table of len(vocabulary) rows' % name)
+  if input_type_name(pipeline_config) == 'CriteoInput':
+    raise NotImplementedError('feature %s: vocab_list / vocab_file with CriteoInput, whose category columns are '
+                              'integers unpacked on the device' % name)
+  if ftype == 'IdFeature' and field_types.get(fc.input_names[0]) != 'STRING':
+    # input/input.py:536-555 passes such a field on unconverted, and TF's vocabulary column then refuses the integer
+    # tensor (VocabularyListCategoricalColumn._transform_input_tensor: "Column dtype and SparseTensors dtype must be
+    # compatible")
+    raise ValueError('feature %s: vocab_list / vocab_file on the %s field %s; an IdFeature with a vocabulary reads a '
+                     'STRING field' % (name, field_types.get(fc.input_names[0], 'undeclared'), fc.input_names[0]))
+  return vocab_keys(name, entries)
+
+
 def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
   """FeatureConfig protos -> FeatureSpec list (config order = packed feature order)."""
   specs = []
@@ -34,6 +102,8 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
     kv = int(ev.max_capacity) if ev is not None else 0
     if kv and ftype_name(fc) == 'RawFeature' and fc.embedding_dim == 0 and raw_boundaries(fc) is None:
       kv = 0   # a numeric column without a table: ev_params has nothing to apply to
+    # a vocabulary column: the readers key its strings, K1 finds their entries (ER_BUCKET_VOCAB)
+    vocab = vocabulary(pipeline_config, fc, name, field_types, kv)
     if kv and (ftype_name(fc) not in ('IdFeature', 'TagFeature') or raw_boundaries(fc) is not None or
                (fc.hash_bucket_size <= 0 and fc.num_buckets <= 0)):
       raise NotImplementedError('feature %s: ev_params (key-value tables) on a %s; only IdFeatures and TagFeatures '
@@ -43,7 +113,6 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
     host_hashed = fc.hash_bucket_size > 0 and field_types.get(fc.input_names[0]) == 'STRING'
     # per-feature options that change which row / value a sample reads and are not implemented: refuse
     unsupported = [w for w, on in (
-        ('vocab_file / vocab_list (vocabulary lookup)', fc.HasField('vocab_file') or len(fc.vocab_list) > 0),
         ('kv_separator on a feature that is not a TagFeature', fc.HasField('kv_separator') and ftype_name(fc) != 'TagFeature'),
         ('seq_multi_sep on a feature that is not a SequenceFeature', fc.HasField('seq_multi_sep') and ftype_name(fc) != 'SequenceFeature'),
         ('normalizer_fn on a feature that is not a RawFeature', fc.HasField('normalizer_fn') and ftype_name(fc) != 'RawFeature'),
@@ -55,7 +124,7 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
       specs.append(IL.id_feature(name, fc.embedding_dim, hash_bucket_size=fc.hash_bucket_size,
                                  num_buckets=fc.num_buckets, combiner=fc.combiner,
                                  embedding_name=fc.embedding_name, packed_mod=packed_mod, host_hashed=host_hashed,
-                                 kv_capacity=kv))
+                                 kv_capacity=kv, vocab=vocab))
     elif ftype == 'ComboFeature':
       # crossed_column over the inputs' string forms (feature_column/feature_column.py:424-455): the reader computes
       # FingerprintCat64 over the inputs' fingerprints % hash_bucket_size (readers.cross_hash); an id slot from there on
@@ -85,10 +154,25 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
                                     combiner=fc.combiner, embedding_name=fc.embedding_name,
                                     seq_len=((fc.max_seq_len if fc.HasField('max_seq_len') else default_seq_len)
                                              if ftype == 'SequenceFeature' else 1),
-                                    packed_mod=packed_mod, host_hashed=host_hashed, kv_capacity=kv))
+                                    packed_mod=packed_mod, host_hashed=host_hashed, kv_capacity=kv, vocab=vocab))
     else:
       raise NotImplementedError('feature_type %s (feature %s) is outside the hot-path scope' % (ftype, name))
+  check_vocab_tables(specs)
   return specs
+
+
+def check_vocab_tables(specs):
+  """features that share an embedding_name read one table: with a vocabulary among them, they must agree on its row
+  count (the reference's shared embedding variable has one shape)"""
+  by_table = collections.defaultdict(list)
+  for sp in specs:
+    if sp.embedding_name:
+      by_table[sp.embedding_name].append(sp)
+  for table, group in by_table.items():
+    if any(sp.vocab is not None for sp in group) and len(set(sp.num_buckets for sp in group)) > 1:
+      raise ValueError('embedding_name %s: shared by features with different row counts (%s); a vocabulary column '
+                       'has len(vocabulary) rows' % (table, ', '.join('%s: %d' % (sp.name, sp.num_buckets)
+                                                                       for sp in group)))
 
 
 def ftype_name(fc):
@@ -431,6 +515,10 @@ def embedding_layer_tables(model_config, specs):
       raise ValueError('embedding_layer block %s takes exactly one feature_group_name input' % b.name)
     for n in groups[b.inputs[0].feature_group_name]:
       sp = specs[by_name[n]]
+      if sp.vocab is not None:
+        raise NotImplementedError('embedding_layer block %s: feature %s has a vocabulary; the block hashes string '
+                                  'features into vocabulary-sized buckets (layers/input_layer.py:222-243) instead of '
+                                  'looking them up, which is not built' % (b.name, n))
       if sp.kind not in ('id', 'tag'):
         raise NotImplementedError('embedding_layer block %s: feature %s is a %s feature; id / bucketized / tag features '
                                   'go through this block' % (b.name, n, sp.kind))

@@ -6,9 +6,12 @@
 //   vals % num_buckets                 input/parquet_input.py:221
 //   identity column with default 0     feature_column_v2.py:4268-4292
 //   uniq % N / int64(recv / N)         compat/feature_column/feature_column.py:296,317
-// Both kernels are pure streaming integer work: 8 B in + 8 B out per lookup.
+//   vocabulary list / file, default 0  feature_column/feature_column.py:277-290,320-333,497-509
+// The hashing kernels are pure streaming integer work: 8 B in + 8 B out per lookup; a vocabulary lookup adds the
+// probe of its index (one or two 128-byte groups at the index's load factor of at most 1/2).
 #include "common.cuh"
 #include "hash.cuh"
+#include "kv_index.cuh"
 #include "scan.cuh"
 #include "slots.cuh"
 
@@ -177,6 +180,73 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// K1 for slot plans with vocabulary slots (ER_BUCKET_VOCAB); kSeq: the un-pooled history form of bucketize_seq_kernel.
+// Each warp walks 32 consecutive lookups together (the loop bound is uniform over the warp, lanes past the end carry
+// nothing), so its two 16-lane tiles are whole when they probe: a tile looks up its lanes' vocabulary keys one after
+// the other, all 16 lanes comparing one 128-byte group of the index per step (kv_find_slot, csrc/kv_index.cuh).
+// Lookups of the other modes take bucket_of as in the kernels above.
+template <bool kSeq>
+__global__ void __launch_bounds__(256)
+    bucketize_vocab_kernel(const int64_t* __restrict__ ids, const float* __restrict__ weights,
+                           const int32_t* __restrict__ seg_ids, const int32_t* __restrict__ row_ptr,
+                           const int32_t* __restrict__ lens, int64_t n_seg, int64_t cap, int T,
+                           const er_slot_t* __restrict__ slots, int n_slots, const er_vocab_t* __restrict__ vocabs,
+                           int64_t* __restrict__ rows, int32_t* __restrict__ owner) {
+  extern __shared__ __align__(16) unsigned char s_raw[];
+  BucketRule* tab = reinterpret_cast<BucketRule*>(s_raw);
+  if constexpr (kSeq) er_pdl_wait();
+  const int uniform = stage_rules(tab, slots, n_slots);
+  const int nseg0 = slots[0].n_seg;
+  const FastDiv div = make_fastdiv((uint32_t)(nseg0 > 0 ? nseg0 : 1));
+  const FastDiv tdiv = make_fastdiv((uint32_t)T);
+  int64_t n = cap;
+  if (!kSeq && row_ptr) {
+    const int64_t total = row_ptr[n_seg];
+    n = total < cap ? total : cap;
+  }
+  const int lane = threadIdx.x & 31, t = lane & (kKvTile - 1), base = lane & kKvTile;
+  const unsigned tmask = 0xFFFFu << base;
+  for (int64_t l0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); l0 < n;
+       l0 += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t l = l0 + lane;
+    bool live = l < n;
+    int32_t s = (int32_t)l;
+    if (live) {
+      if constexpr (kSeq) {
+        const uint32_t sample = fastdiv((uint32_t)l, tdiv);
+        if ((int)((uint32_t)l - sample * (uint32_t)T) >= lens[sample]) {   // a padded step: its id is not read
+          rows[l] = -1;
+          if (owner) owner[l] = -1;
+          live = false;
+        }
+      } else if (seg_ids) {
+        s = seg_ids[l];
+      }
+    }
+    const int f = live ? slot_rule(tab, n_slots, uniform, div, s) : 0;
+    const int64_t v = live ? ids[l] : -1;
+    const bool vocab = live && tab[f].mode == ER_BUCKET_VOCAB;
+    bool drop = vocab && v < 0;
+    int64_t r = 0;
+    if (live && !vocab) r = bucket_of(tab[f], v, drop);
+    // the tile's vocabulary keys, one at a time: a hit reads the entry's position, a miss row 0 (default_value 0)
+    unsigned todo = (__ballot_sync(tmask, vocab && v >= 0) >> base) & 0xFFFFu;
+    while (todo) {
+      const int j = __ffs(todo) - 1;
+      todo &= todo - 1;
+      const int64_t k = __shfl_sync(tmask, v, base + j);
+      const er_vocab_t vb = vocabs[__shfl_sync(tmask, f, base + j)];
+      const KvIndex ix{(long long*)vb.index_keys, (int64_t*)vb.index_rows, vb.n_index / kKvTile};
+      const int64_t e = kv_find_slot(ix, k, t, base, tmask);
+      if (t == j) r = e >= 0 ? vb.index_rows[e] : 0;
+    }
+    if (!live) continue;
+    const BucketRule& rule = tab[f];
+    if (!kSeq && weights && rule.combiner != ER_COMBINER_SUM && !(weights[l] > 0.f)) drop = true;
+    store_row(rule, r, drop, l, rows, owner);
+  }
+}
+
 }  // namespace er
 
 extern "C" size_t er_csr_workspace_bytes(int64_t n_seg) {
@@ -240,6 +310,41 @@ extern "C" int er_bucketize_seq(const int64_t* ids, const int32_t* lens, int64_t
   ER_REQUIRE(n_steps < (1LL << 31), "n_features * batch * seq_len must fit 31 bits");
   launch_pdl(bucketize_seq_kernel, dim3(grid_for(n_steps, 256, 8)), dim3(256), (size_t)n_slots * sizeof(BucketRule),
              as_stream(stream), ids, lens, n_steps, (int)seq_len, slots, (int)n_slots, rows, owner);
+  count_launches(1);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_bucketize_vocab(const int64_t* ids, const float* weights, const int32_t* seg_ids,
+                                  const int32_t* row_ptr, int64_t n_seg, int64_t n_lookups_cap,
+                                  const er_slot_t* slots, int32_t n_slots, const er_vocab_t* vocabs, int64_t* rows,
+                                  int32_t* owner, er_stream_t stream) {
+  using namespace er;
+  ER_REQUIRE(ids && rows && slots && vocabs, "ids, rows, slots and vocabs must be non-null");
+  ER_REQUIRE(n_slots > 0 && n_slots <= 1024, "n_slots must be in [1, 1024]");
+  ER_REQUIRE(n_lookups_cap >= 0 && n_lookups_cap < (1LL << 31), "n_lookups_cap out of range");
+  if (n_lookups_cap == 0) return ER_OK;
+  bucketize_vocab_kernel<false><<<grid_for(n_lookups_cap, 256, 8), 256, (size_t)n_slots * sizeof(BucketRule),
+                                  as_stream(stream)>>>(ids, weights, seg_ids, row_ptr, nullptr, n_seg, n_lookups_cap, 1,
+                                                       slots, n_slots, vocabs, rows, owner);
+  count_launches(1);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_bucketize_seq_vocab(const int64_t* ids, const int32_t* lens, int64_t batch, int32_t seq_len,
+                                      int32_t n_features, const er_slot_t* slots, int32_t n_slots,
+                                      const er_vocab_t* vocabs, int64_t* rows, int32_t* owner, er_stream_t stream) {
+  using namespace er;
+  ER_REQUIRE(ids && lens && rows && slots && vocabs, "ids, lens, rows, slots and vocabs must be non-null");
+  ER_REQUIRE(n_slots > 0 && n_slots <= 1024, "n_slots must be in [1, 1024]");
+  ER_REQUIRE(batch > 0 && seq_len > 0 && n_features > 0, "batch, seq_len and n_features must be positive");
+  const int64_t n_steps = (int64_t)n_features * batch * seq_len;
+  ER_REQUIRE(n_steps < (1LL << 31), "n_features * batch * seq_len must fit 31 bits");
+  launch_pdl(bucketize_vocab_kernel<true>, dim3(grid_for(n_steps, 256, 8)), dim3(256),
+             (size_t)n_slots * sizeof(BucketRule), as_stream(stream), ids, (const float*)nullptr,
+             (const int32_t*)nullptr, (const int32_t*)nullptr, lens, n_steps, n_steps, (int)seq_len, slots,
+             (int)n_slots, vocabs, rows, owner);
   count_launches(1);
   ER_CUDA_LAUNCH_CHECK();
   return ER_OK;

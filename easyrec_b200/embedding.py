@@ -37,6 +37,7 @@ class Slot(object):
     # True: whatever weights array accompanies the call holds 1.0 for this slot's lookups (plain id / sequence slots
     # next to raw-value slots): the backward skips the per-lookup weight read (ER_COMBINER_UNIT_WEIGHTS)
     self.unit_weights = False
+    self.vocab = None             # Vocab of an ER_BUCKET_VOCAB slot
 
 
 class Arena(object):
@@ -199,6 +200,22 @@ class KvTable(object):
       raise _lib.ErError('key-value table %s: restored keys are negative or repeated' % self.name)
 
 
+class Vocab(object):
+  """A vocabulary column's entries on the device: the read-only index K1 probes for ER_BUCKET_VOCAB slots, built once
+  with the key-value tables' bulk insert (csrc/kv_table.cu layout).  keys[i] = Fingerprint64(entry i) % (2^63 - 1),
+  the key the readers give the feature's raw strings; entry i is row i of the column's table.  The keys must be
+  distinct and >= 0 (builder.vocab_keys refuses other vocabularies by name)."""
+
+  def __init__(self, name, keys, device):
+    self.name = name
+    self.keys = np.asarray(keys, dtype=np.int64)
+    if os.environ.get('ER_PLAN_ONLY') == '1' and not str(device).startswith('cuda'):
+      # a plan built to be inspected, not run (Arena.materialize): no index, and nothing may probe it
+      self.index_keys = self.index_rows = torch.full((16,), _lib.KV_EMPTY, dtype=torch.int64, device=device)
+      return
+    self.index_keys, self.index_rows = K.vocab_index(self.keys, device)
+
+
 class ArenaCall(object):
   """The static plan of one fused lookup over an arena for a fixed batch size:
   slot descriptors on the device, output matrices, backward workspace."""
@@ -233,6 +250,8 @@ class ArenaCall(object):
     self.slots_np = K.make_slots(recs, dim)
     self.slots_dev = K.slots_to_device(self.slots_np, arena.device)
     self.n_slots = len(recs)
+    # the vocabularies of the call's ER_BUCKET_VOCAB slots, handed to every K1 of the call (None: no such slot)
+    self.vocabs = K.vocab_plan(self.slots_np, [s.vocab for s in slots], arena.device)
     self.single_valued = single_valued
     self.max_lookups = self.n_seg if single_valued else int(max_lookups)
     self.needs_scale = any((s.combiner & 0xf) != _lib.COMBINER_SUM for s in slots)

@@ -72,6 +72,13 @@ def cross_hash(fingerprints, num_buckets, hash_key=CROSS_HASH_KEY):
   return (h % np.uint64(num_buckets)).astype(np.int64)
 
 
+def string_keys(values):
+  """strings -> the 63-bit keys of a vocabulary column, Fingerprint64(bytes) % (2^63 - 1), as the CSV parser keys them
+  (er_csv_parse with hash_mod 2^63 - 1); '' and nulls -> -1, the ignored value of string columns
+  (feature_column_v2.py:2566-2585)"""
+  return np.array([_lib.fingerprint64(v) % _lib.KV_BUCKETS if v else -1 for v in values], np.int64)
+
+
 def fingerprint_i64(values):
   """Fingerprint64 of the decimal text of int64 values (tf.as_string first, input/input.py:356-376)."""
   v = np.ascontiguousarray(values, np.int64)
@@ -264,6 +271,11 @@ class CSVInput(object):
         assert input_layer.features[name].bucket_mode in (_lib.BUCKET_IDENTITY, _lib.BUCKET_MOD), \
             'feature %s: the table plan must take host-hashed buckets (builder.feature_specs)' % name
         self.hash_buckets[name] = input_layer.features[name].num_buckets   # (2^63 - 1 for a key-value table)
+      elif name in input_layer.features and input_layer.features[name].bucket_mode == _lib.BUCKET_VOCAB:
+        # a vocabulary column: every raw string becomes its 63-bit key, Fingerprint64 % (2^63 - 1), the same transform
+        # as a key-value table's strings; Tag / Sequence fields are read as strings whatever their declared type
+        # (input/input.py:118-124)
+        self.hash_buckets[name] = _lib.KV_BUCKETS
 
   def _token(self, x, feature):
     """one id token -> int64: Fingerprint64 % hash_bucket_size for a host-hashed STRING field ('' -> -1, the
@@ -747,6 +759,9 @@ class ParquetInput(object):
       elif lens is None and np.asarray(vals).dtype.kind in 'OUS':
         # string column of a hashed feature: bucket on the host like the CSV reader ('' / null -> -1)
         f = il.features[name]
+        if f.bucket_mode == _lib.BUCKET_VOCAB:
+          ids.append(string_keys(vals))
+          continue
         if f.bucket_mode != _lib.BUCKET_IDENTITY:
           raise ValueError('feature %r: string column %r needs a hash_bucket_size and a STRING input field'
                            % (name, self.feature_inputs[name]))
@@ -778,6 +793,11 @@ class ParquetInput(object):
         v, l = bucketize_raw_multi(vals, self.bucketized[f.name])
         tag[f.name] = (torch.from_numpy(v), torch.from_numpy(l), None)
         continue
+      if f.bucket_mode == _lib.BUCKET_VOCAB:
+        if np.asarray(vals).dtype.kind not in 'OUS':
+          raise ValueError('feature %r: a vocabulary feature reads strings; column %r holds %s'
+                           % (f.name, self.feature_inputs[f.name], np.asarray(vals).dtype))
+        vals = string_keys(vals)
       vals = np.array(vals, np.int64)   # owned, writable copy (arrow buffers are read-only)
       if lens is None:
         lens = np.ones(n, np.int32)

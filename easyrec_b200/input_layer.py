@@ -35,11 +35,15 @@ FeatureSpec = collections.namedtuple(
     ['name', 'kind',            # 'id' | 'raw' | 'tag' | 'seq'
      'embedding_dim', 'bucket_mode', 'num_buckets', 'combiner', 'embedding_name',
      'min_val', 'max_val', 'raw_input_dim', 'seq_len',
-     'kv_capacity'],            # > 0: a key-value table (ev_params) of that many rows per rank
-    defaults=(0,))
+     'kv_capacity',             # > 0: a key-value table (ev_params) of that many rows per rank
+     'vocab'],                  # a vocabulary column: the 63-bit key of each entry, entry i = row i (else None)
+    defaults=(0, None))
 
 
-def _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed=False):
+def _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed=False, vocab=None):
+  if vocab is not None:
+    # vocabulary column: the reader's 63-bit key of the raw string -> the position of its entry, 0 when it has none
+    return _lib.BUCKET_VOCAB, len(vocab)
   if hash_bucket_size > 0:
     if host_hashed:
       # string-typed field: the reader already computed Fingerprint64(bytes) % hash_bucket_size (er_csv_parse),
@@ -60,14 +64,19 @@ def _kv_buckets(hash_bucket_size, num_buckets, kv_capacity):
 
 
 def id_feature(name, embedding_dim, hash_bucket_size=0, num_buckets=0, combiner='sum',
-               embedding_name='', packed_mod=False, host_hashed=False, kv_capacity=0):
+               embedding_name='', packed_mod=False, host_hashed=False, kv_capacity=0, vocab=None):
   """IdFeature: hash_bucket_size -> Fingerprint64(as_string) % size; num_buckets -> identity
   (feature_column/feature_column.py:259-300).  packed_mod: the Parquet packed rule
   `vals % num_buckets` (input/parquet_input.py:221).  kv_capacity > 0: a key-value table (ev_params) of that many
-  rows per rank instead of a fixed-size one."""
+  rows per rank instead of a fixed-size one.  vocab: the entries' keys of a vocabulary column (builder.vocab_keys)."""
   hash_bucket_size, num_buckets = _kv_buckets(hash_bucket_size, num_buckets, kv_capacity)
-  mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed)
-  return FeatureSpec(name, 'id', embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1, 1, int(kv_capacity))
+  mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed, vocab)
+  return FeatureSpec(name, 'id', embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1, 1, int(kv_capacity),
+                     _vocab_tuple(vocab))
+
+
+def _vocab_tuple(vocab):
+  return None if vocab is None else tuple(int(k) for k in vocab)
 
 
 def raw_feature(name, embedding_dim=0, min_val=0.0, max_val=0.0, raw_input_dim=1):
@@ -81,15 +90,15 @@ def raw_feature(name, embedding_dim=0, min_val=0.0, max_val=0.0, raw_input_dim=1
 
 
 def multi_feature(name, kind, embedding_dim, hash_bucket_size=0, num_buckets=0, combiner='sum',
-                  embedding_name='', seq_len=1, packed_mod=False, host_hashed=False, kv_capacity=0):
+                  embedding_name='', seq_len=1, packed_mod=False, host_hashed=False, kv_capacity=0, vocab=None):
   """TagFeature (kind 'tag': multi-valued, pooled by `combiner`, optional kv weights;
   feature_column/feature_column.py:301-360) or SequenceFeature (kind 'seq': un-pooled [B,T,D];
-  feature_column_v2.py:4988-5002)."""
+  feature_column_v2.py:4988-5002).  vocab: as in id_feature."""
   assert kind in ('tag', 'seq')
   hash_bucket_size, num_buckets = _kv_buckets(hash_bucket_size, num_buckets, kv_capacity)
-  mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed)
+  mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed, vocab)
   return FeatureSpec(name, kind, embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1,
-                     max(int(seq_len), 1), int(kv_capacity))
+                     max(int(seq_len), 1), int(kv_capacity), _vocab_tuple(vocab))
 
 
 _COMBINER = {'sum': _lib.COMBINER_SUM, 'mean': _lib.COMBINER_MEAN, 'sqrtn': _lib.COMBINER_SQRTN}
@@ -222,6 +231,7 @@ class InputLayer(object):
     self.seqc_order = {}      # group -> names of its sequence-combiner features in config order
     self._shard = (shard_n, shard_rank)
     self._table_kv = {}       # (dim, table) -> the kv_capacity of its readers (0: a static table)
+    self._vocabs = {}         # vocabulary keys -> embedding.Vocab (the index K1 probes)
     for gname, g in groups.items():
       self._plan_group(gname, g, dense_generator)
     for sname, maps in self.seq_att_groups.items():
@@ -306,6 +316,8 @@ class InputLayer(object):
     slot = E.Slot(out_key + '/' + fname, table, f.bucket_mode, f.num_buckets, comb, out_buf=out_key,
                   n_seg_per_sample=f.seq_len if kind in ('seq', 'mseq') else 1)
     slot.out_key = out_key
+    if f.vocab is not None:
+      slot.vocab = self._vocab_index(fname)
     # id and sequence slots never carry per-lookup weights (raw-value and kv-weighted tag slots do)
     slot.unit_weights = f.kind != 'raw' and kind in ('single', 'seq', 'mseq')
     if f.kind == 'raw':
@@ -318,6 +330,14 @@ class InputLayer(object):
       src = ('id', self.sparse_names.index(fname))
     sc.items.append((out_key, fname, slot, src))
     return slot
+
+  def _vocab_index(self, fname):
+    """the device index of feature fname's vocabulary, built once (features with the same vocabulary share it)"""
+    keys = self.features[fname].vocab
+    v = self._vocabs.get(keys)
+    if v is None:
+      v = self._vocabs[keys] = E.Vocab(fname, keys, self.device)
+    return v
 
   def _plan_group(self, gname, g, dense_generator):
     """the columns of one feature group, in config order"""
@@ -708,7 +728,8 @@ class InputLayer(object):
         hit = self._preset_rows.get(key)
         if hit is None:
           cids, w = self._gather_inputs(dim, features.get('sparse_fea'), dense_norm)
-          rows = K.bucketize(cids, call.slots_dev, call.n_slots, call.n_seg, rows=self._rows_buf(key, call))
+          rows = K.bucketize(cids, call.slots_dev, call.n_slots, call.n_seg, rows=self._rows_buf(key, call),
+                            **K.k1_vocab_args(call))
           hit = (rows, w)
           self._preset_rows[key] = hit
         out.append((dim, self.merged[dim], hit[0], hit[1]))
@@ -887,7 +908,8 @@ class InputLayer(object):
       hit = self._rows_cache.get(key)
       if hit is None:
         cids, w = self._gather_inputs(dim, features.get('sparse_fea'), dense_norm)
-        rows = K.bucketize(cids, call.slots_dev, call.n_slots, call.n_seg, rows=self._rows_buf(key, call))
+        rows = K.bucketize(cids, call.slots_dev, call.n_slots, call.n_seg, rows=self._rows_buf(key, call),
+                            **K.k1_vocab_args(call))
         self._rows_cache[key] = (rows, w)
       else:
         rows, w = hit
@@ -923,7 +945,7 @@ class InputLayer(object):
         pad_list.append((pos >= lens[:, None]).reshape(-1))
       ids = ids_list[0] if len(ids_list) == 1 else torch.cat(ids_list)
       pad = pad_list[0] if len(pad_list) == 1 else torch.cat(pad_list)
-      rows = K.bucketize(ids.contiguous(), call.slots_dev, call.n_slots, call.n_seg)
+      rows = K.bucketize(ids.contiguous(), call.slots_dev, call.n_slots, call.n_seg, **K.k1_vocab_args(call))
       rows.masked_fill_(pad, -1)   # positions >= seq_len: empty segment -> zero vector
       outs = E.fused_lookup(call, rows)
       return rows, None, None, None, outs
@@ -933,7 +955,7 @@ class InputLayer(object):
     row_ptr, seg_ids = K.csr_from_lens(lens.contiguous(), cap)
     rows = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
     K.bucketize(ids_cap, call.slots_dev, call.n_slots, call.n_seg, seg_ids=seg_ids, row_ptr=row_ptr,
-                rows=rows, **K.k1_weight_args(ids_cap, weights))
+                rows=rows, **K.k1_vocab_args(call), **K.k1_weight_args(ids_cap, weights))
     rows = self._kv_rows(call.arena, rows, torch.empty_like(rows))
     outs = E.fused_lookup(call, rows, weights=weights, row_ptr=row_ptr)
     return rows, weights, row_ptr, seg_ids, outs

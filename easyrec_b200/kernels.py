@@ -96,10 +96,55 @@ def csr_from_lens(lens, n_lookups_cap, want_seg_ids=True):
   return row_ptr, seg_ids
 
 
+def vocab_index(keys, device):
+  """A vocabulary's read-only index on the device: er_kv_insert_rows of entry i's key with row i into an empty index of
+  at least twice as many slots.  keys: int64 numpy, distinct and >= 0.  Returns (index_keys, index_rows).  K1 probes
+  the index on the GPU; there is no host K1 to read it, so a host device is refused."""
+  if not str(device).startswith('cuda'):
+    raise NotImplementedError('a vocabulary index is probed by K1 on the GPU; device %s has no K1' % device)
+  n_index = 16
+  while n_index < 2 * keys.size:
+    n_index *= 2
+  index_keys = torch.full((n_index,), _lib.KV_EMPTY, dtype=torch.int64, device=device)
+  index_rows = torch.full((n_index,), -1, dtype=torch.int64, device=device)
+  stats = torch.zeros(2, dtype=torch.int64, device=device)
+  kv_insert_rows(index_keys, index_rows, torch.from_numpy(keys).to(device),
+                 torch.arange(keys.size, dtype=torch.int64).to(device), stats)
+  if int(stats[1]):
+    raise _lib.ErError('vocabulary index: %d keys are negative or repeated' % int(stats[1]))
+  return index_keys, index_rows
+
+
+class VocabPlan(object):
+  """The vocabularies of one slot plan: `per_slot[i]` is slot i's embedding.Vocab (None for a slot of another mode);
+  `dev` holds their er_vocab_t descriptors in slot order, the array the *_vocab forms of K1 are given."""
+
+  def __init__(self, per_slot, device):
+    self.per_slot = list(per_slot)
+    desc = np.zeros(len(self.per_slot), dtype=_lib.VOCAB_DTYPE)
+    for i, v in enumerate(self.per_slot):
+      if v is not None:
+        desc[i] = (v.index_keys.data_ptr(), v.index_rows.data_ptr(), v.index_keys.numel())
+    self.dev = torch.from_numpy(desc.view(np.uint8).copy()).to(device)
+
+
+def vocab_plan(slots_np, vocabs, device):
+  """VocabPlan of a slot plan whose slot i reads vocabulary vocabs[i], or None when no slot is ER_BUCKET_VOCAB.  A
+  vocabulary slot without its index is an error: the hashing kernels would read its keys as rows."""
+  modes = [int(m) for m in slots_np['bucket_mode']]
+  if _lib.BUCKET_VOCAB not in modes:
+    return None
+  for i, m in enumerate(modes):
+    if (m == _lib.BUCKET_VOCAB) != (vocabs[i] is not None):
+      raise _lib.ErError('slot %d: a vocabulary goes with bucket mode ER_BUCKET_VOCAB and only with it' % i)
+  return VocabPlan(vocabs, device)
+
+
 def bucketize(ids, slots_dev, n_slots, n_seg, seg_ids=None, row_ptr=None, rows=None,
-              owner=None, weights=None):
+              owner=None, weights=None, vocabs=None):
   """K1 (er_bucketize).  weights: the lookup weights the lookup will be pooled with (er_bucketize_weighted); mean /
-  sqrtn lookups whose weight is not > 0 come out as dropped rows (-1), as safe_embedding_lookup_sparse prunes them."""
+  sqrtn lookups whose weight is not > 0 come out as dropped rows (-1), as safe_embedding_lookup_sparse prunes them.
+  vocabs: the VocabPlan of a plan with vocabulary slots (er_bucketize_vocab)."""
   lib = _lib.load()
   _chk(ids, torch.int64, 'ids')
   _chk(weights, torch.float32, 'weights')
@@ -109,6 +154,12 @@ def bucketize(ids, slots_dev, n_slots, n_seg, seg_ids=None, row_ptr=None, rows=N
   if rows is None:
     rows = torch.empty_like(ids)
   _chk(rows, torch.int64, 'rows')
+  if vocabs is not None:
+    assert len(vocabs.per_slot) == n_slots and (weights is None or weights.numel() >= ids.numel())
+    _lib.check(
+        lib.er_bucketize_vocab(_p(ids), _p(weights), _p(seg_ids), _p(row_ptr), n_seg, ids.numel(), _p(slots_dev),
+                               n_slots, _p(vocabs.dev), _p(rows), _p(owner), _stream()), 'er_bucketize_vocab')
+    return rows
   if weights is None:
     _lib.check(
         lib.er_bucketize(_p(ids), _p(seg_ids), _p(row_ptr), n_seg, ids.numel(), _p(slots_dev),
@@ -121,9 +172,10 @@ def bucketize(ids, slots_dev, n_slots, n_seg, seg_ids=None, row_ptr=None, rows=N
   return rows
 
 
-def bucketize_seq(ids, lens, batch, seq_len, slots_dev, n_slots, rows=None, owner=None):
+def bucketize_seq(ids, lens, batch, seq_len, slots_dev, n_slots, rows=None, owner=None, vocabs=None):
   """K1 over un-pooled histories (er_bucketize_seq): ids int64 [n_features * batch * seq_len] steps, lens int32
-  [n_features * batch].  Steps at or beyond their sample's length come out as rows = owner = -1."""
+  [n_features * batch].  Steps at or beyond their sample's length come out as rows = owner = -1.  vocabs: as in
+  bucketize (er_bucketize_seq_vocab)."""
   lib = _lib.load()
   _chk(ids, torch.int64, 'ids')
   _chk(lens, torch.int32, 'lens')
@@ -134,6 +186,12 @@ def bucketize_seq(ids, lens, batch, seq_len, slots_dev, n_slots, rows=None, owne
     rows = torch.empty_like(ids)
   _chk(rows, torch.int64, 'rows')
   assert rows.numel() == ids.numel() and (owner is None or owner.numel() == ids.numel())
+  if vocabs is not None:
+    assert len(vocabs.per_slot) == n_slots
+    _lib.check(
+        lib.er_bucketize_seq_vocab(_p(ids), _p(lens), int(batch), int(seq_len), n_features, _p(slots_dev), n_slots,
+                                   _p(vocabs.dev), _p(rows), _p(owner), _stream()), 'er_bucketize_seq_vocab')
+    return rows
   _lib.check(
       lib.er_bucketize_seq(_p(ids), _p(lens), int(batch), int(seq_len), n_features, _p(slots_dev), n_slots, _p(rows),
                            _p(owner), _stream()), 'er_bucketize_seq')
@@ -185,6 +243,12 @@ def k1_weight_args(ids, weights):
   pooling prunes are dropped before K7, er_mark_rows and K8 see them.  Only device tensors take this path: the host
   runs of the input layer (tests/host_doubles.py) stand in for K1 with a double whose bucketize takes no weights."""
   return {'weights': weights} if weights is not None and ids.is_cuda else {}
+
+
+def k1_vocab_args(call):
+  """Keyword arguments of bucketize() / bucketize_seq() that hand a call's vocabularies to K1 (none for a call without
+  vocabulary slots, so that the calls of such plans stay what they were)."""
+  return {'vocabs': call.vocabs} if getattr(call, 'vocabs', None) is not None else {}
 
 
 def dropout(x, rate, seed, counter, out=None):

@@ -121,14 +121,15 @@ class ShardedExchange(object):
     """K1 of launch m into its range `rows` / `owner`"""
     call = m.call
     if p.lens is not None:
-      K.bucketize_seq(ids, p.lens, m.seq[0], m.seq[1], call.slots_dev, call.n_slots, rows=rows, owner=owner)
+      K.bucketize_seq(ids, p.lens, m.seq[0], m.seq[1], call.slots_dev, call.n_slots, rows=rows, owner=owner,
+                      **K.k1_vocab_args(call))
       return
     if m.csr:
       # multi-valued slots: K1 writes the real lookups only; the padding of the fixed-capacity range asks for nothing
       rows.fill_(-1)
       owner.fill_(-1)
     K.bucketize(ids, call.slots_dev, call.n_slots, call.n_seg, seg_ids=p.seg_ids, row_ptr=p.row_ptr, rows=rows,
-                owner=owner, **K.k1_weight_args(ids, p.weights))
+                owner=owner, **K.k1_weight_args(ids, p.weights), **K.k1_vocab_args(call))
 
   def prefetch(self, inputs):
     """The id half of the NEXT batch's exchange (K1 of every launch -> K8 -> all_to_all(ids)), on a side stream beside

@@ -59,7 +59,13 @@ typedef enum er_bucket_mode {
    * input/input.py:648-673: id 0 weighted by the value) and no other slot of the call reads it:
    * every value >= 0 maps to that row, < 0 is dropped.  er_embedding_bwd does not send these lookups
    * through the dedup: the row's gradient is the weighted column sum of the slot's gradient block. */
-  ER_BUCKET_ONE_ROW = 4
+  ER_BUCKET_ONE_ROW = 4,
+  /* vocabulary column (categorical_column_with_vocabulary_{list,file} with default_value 0 and no OOV buckets,
+   * feature_column/feature_column.py:277-290,320-333,497-509): v is the 63-bit key of the raw string
+   * (Fingerprint64(bytes) % (2^63 - 1)); row = the position of the vocabulary entry with key v, 0 when no entry
+   * has it; v < 0 dropped.  num_buckets = the vocabulary's size.  The entries live in a read-only index
+   * (er_vocab_t) that only the *_vocab forms of K1 are given. */
+  ER_BUCKET_VOCAB = 5
 } er_bucket_mode;
 
 /* safe_embedding_lookup_sparse combiners (compat/embedding_ops.py:37-162,
@@ -185,6 +191,29 @@ int er_bucketize_seq(const int64_t* ids, const int32_t* lens, int64_t batch,
                      int32_t seq_len, int32_t n_features, const er_slot_t* slots,
                      int32_t n_slots, int64_t* rows, int32_t* owner,
                      er_stream_t stream);
+
+/* A vocabulary's index for ER_BUCKET_VOCAB slots: the layout of a key-value table's index (ER_KV_EMPTY = free
+ * entry, n_index a power of two >= 16), built once with er_kv_insert_rows from the entries' keys and their
+ * positions, and never written after.  DEVICE memory, like the arrays it points to. */
+typedef struct er_vocab {
+  const int64_t* index_keys;
+  const int64_t* index_rows;
+  int64_t n_index;
+} er_vocab_t;
+
+/* er_bucketize_weighted for slot plans with ER_BUCKET_VOCAB slots: vocabs (DEVICE, n_slots entries) holds slot i's
+ * vocabulary at vocabs[i] (the entries of other slots are not read).  A hit reads the entry's position, a miss
+ * row 0, a key < 0 is dropped; then row_offset, shard_n and the weight pruning apply as for every other mode.  Every
+ * other slot gives er_bucketize_weighted's result bit for bit.  One launch. */
+int er_bucketize_vocab(const int64_t* ids, const float* weights, const int32_t* seg_ids,
+                       const int32_t* row_ptr, int64_t n_seg, int64_t n_lookups_cap,
+                       const er_slot_t* slots, int32_t n_slots, const er_vocab_t* vocabs,
+                       int64_t* rows, int32_t* owner, er_stream_t stream);
+/* er_bucketize_seq with vocabularies, as er_bucketize_vocab; padded steps are -1 and their ids are not read. */
+int er_bucketize_seq_vocab(const int64_t* ids, const int32_t* lens, int64_t batch,
+                           int32_t seq_len, int32_t n_features, const er_slot_t* slots,
+                           int32_t n_slots, const er_vocab_t* vocabs, int64_t* rows,
+                           int32_t* owner, er_stream_t stream);
 
 /* ---- K8: index bucketing of the row-sharded lookup --------------------
  * Replaces the Unique + dynamic_partition + host-read split sizes of

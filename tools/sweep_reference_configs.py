@@ -3,6 +3,8 @@ Needs /root/reference.   python tools/sweep_reference_configs.py"""
 import glob, os, sys, collections, traceback
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
+# the plans are built, not trained: tables are allocated but not initialised, and vocabularies get no device index
+os.environ.setdefault('ER_PLAN_ONLY', '1')
 from easyrec_b200 import builder
 from easyrec_b200.config import config_util
 REF='/root/reference'
