@@ -180,6 +180,8 @@ SIGNATURES = {
     'er_bias_bn_act_bwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                    c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp,
                                    c_vp, c_sz, c_vp]),
+    'er_bn_relu_bwd': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp,
+                               c_vp, c_sz, c_vp]),
     'er_din_concat_fwd': (c_i32, [c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     'er_din_concat_bwd': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp]),
     'er_din_pool_fwd': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp]),

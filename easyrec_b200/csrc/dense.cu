@@ -9,7 +9,8 @@
 // per-chunk partial statistics (Welford count/mean/M2, merged with Chan's formula in a fixed order
 // -- no atomics, no E[x^2]-E[x]^2 cancellation); pass 2 re-derives the column statistics from the
 // R partials (R*32 L2 reads per CTA) and streams the tile.  Traffic: fwd 2 reads + 1 write of
-// [B,U]; bwd 3 reads (z, y, gy) twice + 1 write.
+// [B,U]; bwd 3 reads (z, y, gy) twice + 1 write.  er_bn_relu_bwd recomputes the relu mask from z (bn_pre_act) instead
+// of reading y: 2 reads (z, gy) twice + 1 write.
 #include <algorithm>
 
 #include "common.cuh"
@@ -146,7 +147,7 @@ __global__ void __launch_bounds__(256)
   const int64_t r0 = (int64_t)blockIdx.y * s.rows_per_chunk;
   const int64_t r1 = min(s.batch, r0 + s.rows_per_chunk);
   for (int64_t r = r0 + rl; r < r1; r += kRowLanes) {
-    const float h = ((z[r * s.units + c] + b) - mean) * rstd * ga + be;
+    const float h = bn_pre_act(z[r * s.units + c], b, mean, rstd, ga, be);
     y[r * s.units + c] = relu ? fmaxf(h, 0.f) : h;
   }
 }
@@ -169,10 +170,10 @@ __global__ void __launch_bounds__(256)
     float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
     if (bias) b = *reinterpret_cast<const float4*>(bias + c);
     float4 h;
-    h.x = ((v.x + b.x) - mu.x) * rs.x * ga.x + be.x;
-    h.y = ((v.y + b.y) - mu.y) * rs.y * ga.y + be.y;
-    h.z = ((v.z + b.z) - mu.z) * rs.z * ga.z + be.z;
-    h.w = ((v.w + b.w) - mu.w) * rs.w * ga.w + be.w;
+    h.x = bn_pre_act(v.x, b.x, mu.x, rs.x, ga.x, be.x);
+    h.y = bn_pre_act(v.y, b.y, mu.y, rs.y, ga.y, be.y);
+    h.z = bn_pre_act(v.z, b.z, mu.z, rs.z, ga.z, be.z);
+    h.w = bn_pre_act(v.w, b.w, mu.w, rs.w, ga.w, be.w);
     if (relu) {
       h.x = fmaxf(h.x, 0.f); h.y = fmaxf(h.y, 0.f); h.z = fmaxf(h.z, 0.f); h.w = fmaxf(h.w, 0.f);
     }
@@ -187,7 +188,7 @@ __global__ void __launch_bounds__(256)
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total;
        t += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(t % units);
-    const float h = ((z[t] + (bias ? bias[c] : 0.f)) - mean[c]) * rstd[c] * gamma[c] + beta[c];
+    const float h = bn_pre_act(z[t], bias ? bias[c] : 0.f, mean[c], rstd[c], gamma[c], beta[c]);
     y[t] = relu ? fmaxf(h, 0.f) : h;
   }
 }
@@ -339,9 +340,20 @@ __device__ __forceinline__ void relu_mask4(float4& g, const float4& yy) {
   if (!(yy.z > 0.f)) g.z = 0.f;
   if (!(yy.w > 0.f)) g.w = 0.f;
 }
+// the same mask from z: y > 0 exactly when the batch-normalised value is (bn_pre_act is the forward's expression)
+__device__ __forceinline__ void relu_mask4_z(float4& g, const float4& zz, const float4& b, const float4& mu,
+                                             const float4& rs, const float4& ga, const float4& be) {
+  if (!(bn_pre_act(zz.x, b.x, mu.x, rs.x, ga.x, be.x) > 0.f)) g.x = 0.f;
+  if (!(bn_pre_act(zz.y, b.y, mu.y, rs.y, ga.y, be.y) > 0.f)) g.y = 0.f;
+  if (!(bn_pre_act(zz.z, b.z, mu.z, rs.z, ga.z, be.z) > 0.f)) g.z = 0.f;
+  if (!(bn_pre_act(zz.w, b.w, mu.w, rs.w, ga.w, be.w) > 0.f)) g.w = 0.f;
+}
 
+// kZMask: batch norm + relu with the mask recomputed from z (gamma, beta given, y not read); else the mask comes from y
+template <bool kZMask>
 __global__ void __launch_bounds__(256)
     bn_bwd_stats_vec_kernel(const float* __restrict__ z, const float* __restrict__ bias,
+                            const float* __restrict__ gamma, const float* __restrict__ beta,
                             const float* __restrict__ y, const float* __restrict__ gy,
                             const float* __restrict__ save_mean, const float* __restrict__ save_rstd,
                             VecShape s, int relu, int use_bn, float* __restrict__ part /* [n_chunks][units][2] */) {
@@ -353,17 +365,25 @@ __global__ void __launch_bounds__(256)
   const int64_t r1 = min(s.batch, r0 + s.rows_per_chunk);
   float4 sg = make_float4(0.f, 0.f, 0.f, 0.f), sx = sg;
   if (c < s.units) {
-    float4 b = make_float4(0.f, 0.f, 0.f, 0.f), mu = b, rs = b;
+    float4 b = make_float4(0.f, 0.f, 0.f, 0.f), mu = b, rs = b, ga = b, be = b;
     if (bias) b = ld4(bias + c);
     if (use_bn) {
       mu = ld4(save_mean + c);
       rs = ld4(save_rstd + c);
     }
+    if (kZMask) {
+      ga = ld4(gamma + c);
+      be = ld4(beta + c);
+    }
 #pragma unroll 4
     for (int64_t r = r0 + rl; r < r1; r += kRowLanes) {
       const int64_t i = r * s.units + c;
       float4 g = ld4(gy + i);
-      if (relu) relu_mask4(g, ld4(y + i));
+      if (kZMask) {
+        if (relu) relu_mask4_z(g, ld4(z + i), b, mu, rs, ga, be);
+      } else if (relu) {
+        relu_mask4(g, ld4(y + i));
+      }
       sg.x += g.x; sg.y += g.y; sg.z += g.z; sg.w += g.w;
       if (use_bn) {
         const float4 zz = ld4(z + i);
@@ -390,12 +410,13 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+template <bool kZMask>
 __global__ void __launch_bounds__(256)
     bn_bwd_apply_vec_kernel(const float* __restrict__ z, const float* __restrict__ bias,
-                            const float* __restrict__ gamma, const float* __restrict__ y,
-                            const float* __restrict__ gy, const float* __restrict__ save_mean,
-                            const float* __restrict__ save_rstd, VecShape s, int relu, int use_bn,
-                            const float* __restrict__ part, float* __restrict__ gz,
+                            const float* __restrict__ gamma, const float* __restrict__ beta,
+                            const float* __restrict__ y, const float* __restrict__ gy,
+                            const float* __restrict__ save_mean, const float* __restrict__ save_rstd, VecShape s,
+                            int relu, int use_bn, const float* __restrict__ part, float* __restrict__ gz,
                             float* __restrict__ gbias, float* __restrict__ ggamma, float* __restrict__ gbeta) {
   er_pdl_wait();
   __shared__ float4 s_a[kRowLanes][32], s_b[kRowLanes][32];
@@ -432,13 +453,14 @@ __global__ void __launch_bounds__(256)
       *reinterpret_cast<float4*>(gbias + c) = sg;
     }
   }
-  float4 b = make_float4(0.f, 0.f, 0.f, 0.f), mu = b, rs = b, ga = make_float4(1.f, 1.f, 1.f, 1.f);
+  float4 b = make_float4(0.f, 0.f, 0.f, 0.f), mu = b, rs = b, be = b, ga = make_float4(1.f, 1.f, 1.f, 1.f);
   if (bias) b = ld4(bias + c);
   if (use_bn) {
     mu = ld4(save_mean + c);
     rs = ld4(save_rstd + c);
     ga = ld4(gamma + c);
   }
+  if (kZMask) be = ld4(beta + c);
   const float inv_b = 1.0f / (float)s.batch;
   const int64_t r0 = (int64_t)blockIdx.y * s.rows_per_chunk;
   const int64_t r1 = min(s.batch, r0 + s.rows_per_chunk);
@@ -446,7 +468,11 @@ __global__ void __launch_bounds__(256)
   for (int64_t r = r0 + rl; r < r1; r += kRowLanes) {
     const int64_t i = r * s.units + c;
     float4 g = ld4(gy + i);
-    if (relu) relu_mask4(g, ld4(y + i));
+    if (kZMask) {
+      if (relu) relu_mask4_z(g, ld4(z + i), b, mu, rs, ga, be);
+    } else if (relu) {
+      relu_mask4(g, ld4(y + i));
+    }
     if (use_bn) {
       const float4 zz = ld4(z + i);
       g.x = ga.x * rs.x * (g.x - sg.x * inv_b - (((zz.x + b.x) - mu.x) * rs.x) * sx.x * inv_b);
@@ -546,10 +572,10 @@ extern "C" int er_bias_bn_act_bwd(const float* z, const float* bias, const float
       (!use_bn || (al(gamma) && al(save_mean) && al(save_rstd) && (!ggamma || al(ggamma)) && (!gbeta || al(gbeta))))) {
     VecShape v = vec_shape(batch, units);
     dim3 vgrid((units + kVecCols - 1) / kVecCols, v.n_chunks);
-    launch_pdl(bn_bwd_stats_vec_kernel, vgrid, dim3(256), 0, st, z, bias, y, gy, save_mean, save_rstd, v, (int)relu,
-               use_bn, part);
-    launch_pdl(bn_bwd_apply_vec_kernel, vgrid, dim3(256), 0, st, z, bias, gamma, y, gy, save_mean, save_rstd, v,
-               (int)relu, use_bn, (const float*)part, gz, gbias, ggamma, gbeta);
+    launch_pdl(bn_bwd_stats_vec_kernel<false>, vgrid, dim3(256), 0, st, z, bias, (const float*)nullptr,
+               (const float*)nullptr, y, gy, save_mean, save_rstd, v, (int)relu, use_bn, part);
+    launch_pdl(bn_bwd_apply_vec_kernel<false>, vgrid, dim3(256), 0, st, z, bias, gamma, (const float*)nullptr, y,
+               gy, save_mean, save_rstd, v, (int)relu, use_bn, (const float*)part, gz, gbias, ggamma, gbeta);
     count_launches(2);
     ER_CUDA_LAUNCH_CHECK();
     return ER_OK;
@@ -557,6 +583,33 @@ extern "C" int er_bias_bn_act_bwd(const float* z, const float* bias, const float
   bn_bwd_stats_kernel<<<grid, 256, 0, st>>>(z, bias, y, gy, save_mean, save_rstd, s, relu, use_bn, part);
   bn_bwd_apply_kernel<<<grid, 256, 0, st>>>(z, bias, gamma, y, gy, save_mean, save_rstd, s, relu, use_bn,
                                             part, gz, gbias, ggamma, gbeta);
+  count_launches(2);
+  ER_CUDA_LAUNCH_CHECK();
+  return ER_OK;
+}
+
+extern "C" int er_bn_relu_bwd(const float* z, const float* bias, const float* gamma, const float* beta,
+                              const float* save_mean, const float* save_rstd, const float* gy, int64_t batch,
+                              int32_t units, int32_t relu, float* gz, float* gbias, float* ggamma, float* gbeta,
+                              void* ws, size_t ws_bytes, er_stream_t stream) {
+  using namespace er;
+  ER_REQUIRE(z && gamma && beta && save_mean && save_rstd && gy && gz, "null argument");
+  ER_REQUIRE(batch > 0 && units > 0, "bad shape");
+  auto al = [](const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; };
+  ER_REQUIRE(units % 4 == 0 && al(z) && al(gamma) && al(beta) && al(save_mean) && al(save_rstd) && al(gy) && al(gz) &&
+                 (!bias || al(bias)) && (!gbias || al(gbias)) && (!ggamma || al(ggamma)) &&
+                 (!gbeta || al(gbeta)),
+             "er_bn_relu_bwd needs units % 4 == 0 and 16-byte aligned arrays");
+  cudaStream_t st = as_stream(stream);
+  VecShape v = vec_shape(batch, units);
+  dim3 vgrid((units + kVecCols - 1) / kVecCols, v.n_chunks);
+  if (!ws || ws_bytes < er_dense_workspace_bytes(batch, units))
+    return fail(ER_ERR_WORKSPACE, "er_bn_relu_bwd: workspace too small");
+  float* part = reinterpret_cast<float*>(static_cast<char*>(ws) + 1024);
+  launch_pdl(bn_bwd_stats_vec_kernel<true>, vgrid, dim3(256), 0, st, z, bias, gamma, beta, (const float*)nullptr, gy,
+             save_mean, save_rstd, v, (int)relu, 1, part);
+  launch_pdl(bn_bwd_apply_vec_kernel<true>, vgrid, dim3(256), 0, st, z, bias, gamma, beta, (const float*)nullptr, gy,
+             save_mean, save_rstd, v, (int)relu, 1, (const float*)part, gz, gbias, ggamma, gbeta);
   count_launches(2);
   ER_CUDA_LAUNCH_CHECK();
   return ER_OK;

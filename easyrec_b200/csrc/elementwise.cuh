@@ -55,6 +55,18 @@ ER_HD float act_slope(float x) {
 }
 
 
+// ---- batch norm of a dense layer, before its relu: h = ((z + b) - mean) * rstd * gamma + beta ----------------------
+// Every kernel that forms h (the forward apply, and the backward passes that recompute the relu mask h > 0 from z instead
+// of reading y) calls this one function, with each rounding spelled out: the mask is then exactly y > 0.  The order is
+// the one nvcc contracted the expression to before (add, sub, mul, then one fma), so y keeps its bits.
+ER_HD float bn_pre_act(float z, float b, float mean, float rstd, float gamma, float beta) {
+#ifdef __CUDA_ARCH__
+  return __fmaf_rn(__fmul_rn(__fsub_rn(__fadd_rn(z, b), mean), rstd), gamma, beta);
+#else
+  return fmaf(((z + b) - mean) * rstd, gamma, beta);
+#endif
+}
+
 // ---- dice (utils/activation.py:13-43, layers/keras/activation.py:24-73): the data-adaptive activation of DIN ------------
 // p = sigmoid(xn), xn = batch_norm(x) without centre / scale (epsilon 1e-9);  y = alpha * (1 - p) * x + p * x.
 // The normalisation itself runs on the batch-norm kernels; these are the gate and its three gradient terms.

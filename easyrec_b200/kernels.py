@@ -938,3 +938,23 @@ def bias_bn_act_bwd(z, bias, gamma, y, gy, save_mean, save_rstd, relu, ws):
                              batch, units, 1 if relu else 0, _p(gz), _p(gbias), _p(ggamma), _p(gbeta),
                              _p(ws), ws.numel(), _stream()), 'er_bias_bn_act_bwd')
   return gz, gbias, ggamma, gbeta
+
+
+def bn_relu_bwd(z, bias, gamma, beta, save_mean, save_rstd, gy, relu, ws):
+  """bias_bn_act_bwd for batch norm (+ relu) with the relu mask recomputed from z (er_bn_relu_bwd: y is not read).
+  Returns (gz, gbias, ggamma, gbeta), or None when the arrays do not suit its vector kernels (units % 4, 16-byte
+  alignment): bias_bn_act_bwd then."""
+  lib = _lib.load()
+  _chk(gy, torch.float32, 'gy')
+  batch, units = z.shape
+  if units % 4 or any(t is not None and t.data_ptr() % 16 for t in (z, bias, gamma, beta, save_mean, save_rstd, gy)):
+    return None
+  gz = torch.empty_like(z)
+  gbias = torch.empty(units, dtype=torch.float32, device=z.device)
+  ggamma = torch.empty(units, dtype=torch.float32, device=z.device)
+  gbeta = torch.empty(units, dtype=torch.float32, device=z.device)
+  _lib.check(
+      lib.er_bn_relu_bwd(_p(z), _p(bias), _p(gamma), _p(beta), _p(save_mean), _p(save_rstd), _p(gy), batch, units,
+                         1 if relu else 0, _p(gz), _p(gbias), _p(ggamma), _p(gbeta), _p(ws), ws.numel(), _stream()),
+      'er_bn_relu_bwd')
+  return gz, gbias, ggamma, gbeta

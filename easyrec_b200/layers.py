@@ -113,14 +113,20 @@ class _DenseBNAct(torch.autograd.Function):
     ctx.relu = relu
     ctx.ws = ws
     ctx.has_bn = gamma is not None
-    ctx.save_for_backward(x, kernel, bias, gamma, z, y, mean, rstd)
+    ctx.save_for_backward(x, kernel, bias, gamma, beta, z, y, mean, rstd)
     return y
 
   @staticmethod
   def backward(ctx, gy):
-    x, kernel, bias, gamma, z, y, mean, rstd = ctx.saved_tensors
-    gz, gbias, ggamma, gbeta = K.bias_bn_act_bwd(z, bias, gamma, y, gy.contiguous(), mean, rstd,
-                                                 ctx.relu, ctx.ws)
+    x, kernel, bias, gamma, beta, z, y, mean, rstd = ctx.saved_tensors
+    gy = gy.contiguous()
+    out = None
+    if ctx.has_bn and mean is not None and z.is_cuda:
+      # the relu mask recomputed from z (exactly y > 0): y is not read
+      out = K.bn_relu_bwd(z, bias, gamma, beta, mean, rstd, gy, ctx.relu, ctx.ws)
+    if out is None:
+      out = K.bias_bn_act_bwd(z, bias, gamma, y, gy, mean, rstd, ctx.relu, ctx.ws)
+    gz, gbias, ggamma, gbeta = out
     # dW goes straight into the optimizer's flat gradient buffer when this kernel is applied once per step
     # (a fresh view object, so AccumulateGrad adopts it instead of cloning)
     kp = ctx.kernel_param

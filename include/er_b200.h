@@ -433,6 +433,13 @@ int er_bias_bn_act_bwd(const float* z, const float* bias, const float* gamma,
                        const float* save_rstd, int64_t batch, int32_t units,
                        int32_t relu, float* gz, float* gbias, float* ggamma,
                        float* gbeta, void* ws, size_t ws_bytes, er_stream_t stream);
+/* The same backward for batch norm + relu (gamma and beta given), with the relu mask recomputed from z - y > 0 exactly
+ * when ((z + bias - mean) * rstd * gamma + beta) > 0 in the forward kernels' rounding - so y is not read.  Two launches
+ * (column sums, then gz), ws: er_dense_workspace_bytes; units % 4 == 0 and every array 16-byte aligned. */
+int er_bn_relu_bwd(const float* z, const float* bias, const float* gamma, const float* beta,
+                   const float* save_mean, const float* save_rstd, const float* gy, int64_t batch, int32_t units,
+                   int32_t relu, float* gz, float* gbias, float* ggamma, float* gbeta, void* ws, size_t ws_bytes,
+                   er_stream_t stream);
 
 /* tf.nn.dropout of DNN.__call__ (layers/dnn.py:77-82): y = x * mask / (1 - rate), mask ~ Bernoulli(1 - rate) per
  * element, a counter-based function of (seed, *counter_dev, element index): element i is kept iff the top 32 bits of
