@@ -42,6 +42,11 @@ ABI_VERSION = 3
 KV_EMPTY = -1                 # ER_KV_EMPTY: a free slot of a key-value table's index
 KV_BUCKETS = 2**63 - 1        # the bucket count of a key-value table's slots: K1 then writes the 63-bit key
 CRITEO_N_DENSE, CRITEO_N_CAT = 13, 26   # ER_CRITEO_N_DENSE / ER_CRITEO_N_CAT: values per sample of a binary part
+# er_expr_op_t / er_expr_t, 16 bytes each: an ExprFeature program's ops and its descriptor (er_expr_eval)
+EXPR_OP_DTYPE = np.dtype([('op', '<i4'), ('arg', '<i4'), ('value', '<f8')], align=True)
+EXPR_DTYPE = np.dtype([('begin', '<i4'), ('n_ops', '<i4'), ('out_col', '<i4'), ('pad_', '<i4')], align=True)
+assert EXPR_OP_DTYPE.itemsize == EXPR_DTYPE.itemsize == 16
+EXPR_MAX_STACK, EXPR_MAX_OPS = 8, 4096   # ER_EXPR_MAX_STACK / ER_EXPR_MAX_OPS
 HYPER_LR, HYPER_BETA1_POWER, HYPER_BETA2_POWER, HYPER_GRAD_SCALE, HYPER_N = 0, 1, 2, 3, 4
 
 
@@ -74,7 +79,7 @@ class ErCsvCol(ctypes.Structure):
 
 ER_OK, ER_ERR_INVALID_ARG, ER_ERR_WORKSPACE, ER_ERR_CUDA, ER_ERR_UNSUPPORTED = range(5)
 CSV_SKIP, CSV_I64, CSV_F32, CSV_HASH, CSV_I64_LIST, CSV_F32_VEC, CSV_HASH_LIST, CSV_I64_KV_LIST, CSV_HASH_KV_LIST, CSV_F32_LIST, \
-    CSV_I64_STEP_LIST, CSV_HASH_STEP_LIST = range(12)
+    CSV_I64_STEP_LIST, CSV_HASH_STEP_LIST, CSV_F64 = range(13)
 
 # name -> (restype, argtypes); must list every symbol include/er_b200.h declares
 SIGNATURES = {
@@ -108,6 +113,7 @@ SIGNATURES = {
     'er_csv_parse_lines': (c_i32, [c_vp, c_sz, ctypes.c_char, ctypes.POINTER(ErCsvCol), c_i32, c_i64, c_i32, c_i64, c_i64,
                                    ctypes.POINTER(c_i64), ctypes.POINTER(c_sz), ctypes.POINTER(c_i64)]),
     'er_fingerprint64_i64': (c_i32, [c_vp, c_i64, c_vp]),
+    'er_expr_eval': (c_i32, [c_vp, c_i64, c_i32, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_i64, c_vp]),
     'er_binary_unpack': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp]),
     'er_load_embed': (c_i32, [ctypes.c_char_p, ctypes.c_char_p, c_i32, c_i32, c_i32, c_i64, c_vp, c_vp]),
     'er_kv_find_or_insert': (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp,

@@ -100,7 +100,8 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
     ev = ev_params(pipeline_config, fc)
     # a key-value table (ev_params): a pool of max_capacity rows per rank, filled as keys are trained
     kv = int(ev.max_capacity) if ev is not None else 0
-    if kv and ftype_name(fc) == 'RawFeature' and fc.embedding_dim == 0 and raw_boundaries(fc) is None:
+    if kv and ((ftype_name(fc) == 'RawFeature' and fc.embedding_dim == 0 and raw_boundaries(fc) is None) or
+               ftype_name(fc) == 'ExprFeature'):
       kv = 0   # a numeric column without a table: ev_params has nothing to apply to
     # a vocabulary column: the readers key its strings, K1 finds their entries (ER_BUCKET_VOCAB)
     vocab = vocabulary(pipeline_config, fc, name, field_types, kv)
@@ -148,6 +149,10 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
                                       combiner=fc.combiner, embedding_name=fc.embedding_name))
     elif ftype == 'RawFeature':
       specs.append(IL.raw_feature(name, fc.embedding_dim, fc.min_val, fc.max_val, fc.raw_input_dim))
+    elif ftype == 'ExprFeature':
+      # numeric_column(shape=(1,)) of the expression's float32 value, not normalised (feature_column/feature_column.py:
+      # 407-422): a raw column without a table, filled on the device by er_expr_eval
+      specs.append(IL.raw_feature(name)._replace(expr=expr_feature(fc, name, field_types)))
     elif ftype in ('TagFeature', 'SequenceFeature'):
       specs.append(IL.multi_feature(name, 'tag' if ftype == 'TagFeature' else 'seq', fc.embedding_dim,
                                     hash_bucket_size=fc.hash_bucket_size, num_buckets=fc.num_buckets,
@@ -159,6 +164,33 @@ def feature_specs(pipeline_config, packed_mod=False, default_seq_len=50):
       raise NotImplementedError('feature_type %s (feature %s) is outside the hot-path scope' % (ftype, name))
   check_vocab_tables(specs)
   return specs
+
+
+_EXPR_FIELD_TYPES = ('INT32', 'INT64', 'FLOAT', 'DOUBLE', 'STRING')
+
+
+def expr_feature(fc, name, field_types):
+  """(expr.Program, input field names) of an ExprFeature.  Its inputs are read as float64 (input/input.py:507-528:
+  STRING fields through string_to_number, the others cast); options the reference never reads for it are refused."""
+  from easyrec_b200 import expr
+  ignored = [w for w, on in (('embedding_dim', fc.embedding_dim > 0), ('boundaries', len(fc.boundaries) > 0),
+                             ('hash_bucket_size', fc.hash_bucket_size > 0)) if on]
+  if ignored:
+    raise NotImplementedError('ExprFeature %s: %s, which the reference ignores for an ExprFeature (a numeric_column of '
+                              'shape (1,), feature_column/feature_column.py:407-422); remove it' % (name, ', '.join(ignored)))
+  if not fc.feature_name:
+    # input/input.py:508 stores the value under fc.feature_name ('' when unset) while parse_expr_feature
+    # (feature_column/feature_column.py:415-418) names the column input_names[0]: the reference would read the raw input
+    # field or fail, never the expression
+    raise ValueError('ExprFeature %s (expression %r) has no feature_name; the reference trains the expression only '
+                     'under its feature_name' % (name, fc.expression))
+  if not fc.HasField('expression'):
+    raise ValueError('ExprFeature %s has no expression' % name)
+  for f in fc.input_names:
+    if field_types.get(f) not in _EXPR_FIELD_TYPES:
+      raise ValueError('ExprFeature %s: input %s is %s; an expression reads INT32, INT64, FLOAT, DOUBLE or STRING '
+                       'fields (input/input.py:513-531)' % (name, f, field_types.get(f, 'not an input field')))
+  return expr.compile_expression(name, fc.expression, list(fc.input_names)), tuple(fc.input_names)
 
 
 def check_vocab_tables(specs):

@@ -123,6 +123,22 @@ inline bool parse_f32(Span s, float* out) {
   return true;
 }
 
+// Correctly rounded decimal -> double (strtod), for ExprFeature inputs.  Hex floats are not decimal numbers.
+inline bool parse_f64(const char* p, size_t n, double* out) {
+  while (n && (*p == ' ' || *p == '\t')) ++p, --n;
+  while (n && (p[n - 1] == ' ' || p[n - 1] == '\t')) --n;
+  char tmp[128];
+  if (n == 0 || n >= sizeof(tmp)) return false;
+  std::memcpy(tmp, p, n);
+  tmp[n] = 0;
+  if (std::strpbrk(tmp, "xX")) return false;
+  char* end = nullptr;
+  const double v = std::strtod(tmp, &end);
+  if (end == tmp || *end != 0) return false;
+  *out = v;
+  return true;
+}
+
 // Fingerprint64 of a string id; with hash_mod the hash bucket (uint64 mod, StringToHashBucketFast) and an
 // empty string -> -1, the "no value" id the lookup drops (feature_column_v2.py:2566-2585 ignores '').
 inline int64_t hashed(const er_csv_col_t& k, const char* p, size_t n) {
@@ -165,7 +181,7 @@ extern "C" int er_csv_parse_lines(const char* buf, size_t len, char sep, er_csv_
   ER_REQUIRE(line_stride >= 1 && line_phase >= 0 && line_phase < line_stride, "bad line_stride / line_phase");
   for (int c = 0; c < n_cols; ++c) {
     const er_csv_col_t& k = cols[c];
-    ER_REQUIRE(k.kind >= ER_CSV_SKIP && k.kind <= ER_CSV_HASH_STEP_LIST, "unknown column kind");
+    ER_REQUIRE(k.kind >= ER_CSV_SKIP && k.kind <= ER_CSV_F64, "unknown column kind");
     ER_REQUIRE(!is_steps(k.kind) || (k.step_lens && k.width > 0 && k.kv_sep), "step-list column needs step_lens, width and the value separator");
     ER_REQUIRE(k.kind == ER_CSV_SKIP || k.out, "column without an output array");
     ER_REQUIRE(!is_list(k.kind) || (k.lens && k.list_cap >= 0), "list column needs lens and list_cap");
@@ -235,7 +251,7 @@ extern "C" int er_csv_parse_lines(const char* buf, size_t len, char sep, er_csv_
     const er_csv_col_t& k = cols[errs[t].col];
     return fail(ER_ERR_INVALID_ARG, "er_csv_parse: line " + std::to_string(line_phase + errs[t].row * line_stride + 1) + ", field " +
                                         std::to_string(errs[t].col + 1) + " is not a valid " +
-                                        (k.kind == ER_CSV_F32 || k.kind == ER_CSV_F32_VEC || k.kind == ER_CSV_F32_LIST ? "float"
+                                        (k.kind == ER_CSV_F32 || k.kind == ER_CSV_F32_VEC || k.kind == ER_CSV_F32_LIST || k.kind == ER_CSV_F64 ? "float"
                                          : is_kv(k.kind)                                  ? "key:weight list"
                                                                                           : "integer"));
   };
@@ -258,6 +274,13 @@ extern "C" int er_csv_parse_lines(const char* buf, size_t len, char sep, er_csv_
           float v = k.default_f32;
           if (s.n && !parse_f32(s, &v)) return c;
           ((float*)k.out)[r] = v;
+          break;
+        }
+        case ER_CSV_F64: {
+          const bool dflt = s.n == 0;
+          if (!parse_f64(dflt ? k.default_str : s.p, dflt ? (k.default_str ? std::strlen(k.default_str) : 0) : s.n,
+                         (double*)k.out + r))
+            return c;
           break;
         }
         case ER_CSV_HASH: {

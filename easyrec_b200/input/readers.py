@@ -168,6 +168,35 @@ def _check_tag_weights(name, lens, wlens):
                      % name)
 
 
+def _expr_inputs(il):
+  """the input fields of the ExprFeatures, columns of the batch's expr_fea (InputLayer.expr_inputs)"""
+  return getattr(il, 'expr_inputs', ())
+
+
+def _expr_features(il):
+  """the ExprFeatures: raw columns the readers leave to er_expr_eval"""
+  return [n for n, f in il.features.items() if getattr(f, 'expr', None) is not None]
+
+
+def expr_number(x, field, ftype, default):
+  """one raw value of an ExprFeature input field -> float64, as input/input.py:507-528 reads it: STRING and DOUBLE
+  fields as decimal numbers (tf.string_to_number(.., tf.float64)), INT fields as integers, FLOAT fields rounded to
+  float32 (the field's parsed type) and then widened.  An empty value takes the field's default_val; '' there is 0 for a
+  number field and not a number for a STRING one.  Raises ValueError naming the field."""
+  x = x if x != '' else (default or ('' if ftype == 'STRING' else '0'))
+  try:
+    t = x.strip(' \t')
+    if '_' in t or 'x' in t or 'X' in t or t != t.strip():
+      raise ValueError(x)
+    if ftype in ('INT32', 'INT64'):
+      return float(int(t))
+    v = float(t)
+    return float(np.float32(v)) if ftype == 'FLOAT' else v
+  except ValueError:
+    raise ValueError('input field %s (%s): %r is not a number; ExprFeature inputs are read with string_to_number'
+                     % (field, ftype, x))
+
+
 class DummyInput(object):
   """input/dummy_input.py:13-58: a constant in-memory batch, for pipeline-free throughput runs and tests."""
 
@@ -186,6 +215,8 @@ class DummyInput(object):
       feats['sparse_fea'] = torch.from_numpy(ids)
     if il.n_dense:
       feats['dense_fea'] = torch.from_numpy(rng.uniform(0, 1, (B, il.n_dense)).astype(np.float32))
+    if _expr_inputs(il):   # small integers: the expressions' comparisons come out both ways, with ties
+      feats['expr_fea'] = torch.from_numpy(rng.integers(0, 10, (B, len(_expr_inputs(il)))).astype(np.float64))
     seq, tag = {}, {}
     for f in il.features.values():
       if f.kind == 'seq' and f.name in getattr(il, 'multi_valued_seq', ()):
@@ -352,10 +383,24 @@ class CSVInput(object):
       else:
         want(src, (_lib.CSV_I64, 0, b',', int(self.defaults.get(src) or 0), 0))
     for n in il.raw_names:
+      if n in _expr_features(il):
+        continue   # (its column is the expression's, filled on the device from expr_fea)
       src, sep = self.feature_inputs[n]
       c0, c1 = il.raw_cols[n]
+      if c1 - c0 == 1 and src in _expr_inputs(il) and self.ftypes[src] in ('INT32', 'INT64', 'DOUBLE'):
+        # the field is also an ExprFeature input: parsed once, as int64 / float64 below, and rounded to float32 for the
+        # raw column - the reference's own cast of an int / double field
+        continue
       d = float(self.defaults.get(src) or 0)
       want(src, (_lib.CSV_F32, 0, b',', d, 0) if c1 - c0 == 1 else (_lib.CSV_F32_VEC, c1 - c0, sep.encode(), d, 0))
+    for src in _expr_inputs(il):
+      t, d = self.ftypes[src], self.defaults.get(src)
+      if t in ('INT32', 'INT64'):
+        want(src, (_lib.CSV_I64, 0, b',', int(d or 0), 0))
+      elif t == 'FLOAT':
+        want(src, (_lib.CSV_F32, 0, b',', float(d or 0), 0))
+      else:   # STRING / DOUBLE: string_to_number(.., float64); an empty STRING default is not a number
+        want(src, (_lib.CSV_F64, 0, b',', d or ('' if t == 'STRING' else '0'), 0))
     for f in il.features.values():
       if f.kind == 'tag' and f.name in self.bucketized:
         src, sep = self.feature_inputs[f.name]
@@ -391,10 +436,10 @@ class CSVInput(object):
       if kind == _lib.CSV_I64:
         c.default_i64 = default
         out[name] = (np.empty(B, np.int64),)
-      elif kind == _lib.CSV_HASH:
+      elif kind in (_lib.CSV_HASH, _lib.CSV_F64):
         keep.append(default.encode())
         c.default_str = keep[-1]
-        out[name] = (np.empty(B, np.int64),)
+        out[name] = (np.empty(B, np.float64 if kind == _lib.CSV_F64 else np.int64),)
       elif kind == _lib.CSV_F32:
         c.default_f32 = default
         out[name] = (np.empty(B, np.float32),)
@@ -424,7 +469,11 @@ class CSVInput(object):
                                         ctypes.byref(seen))
     if st == _lib.ER_ERR_WORKSPACE:
       return None
-    _lib.check(st, 'er_csv_parse_lines')
+    if st != _lib.ER_OK:
+      msg = _lib.load().er_last_error().decode()
+      m = re.search(r'field (\d+) ', msg)
+      raise _lib.ErError('er_csv_parse_lines failed (status %d): %s%s' % (
+          st, msg, ' (input field %s)' % self.fields[int(m.group(1)) - 1] if m else ''))
     for i, name in enumerate(self.fields):
       if cols[i].kind in _STEP_KINDS:
         out[name] = (out[name][0][:cols[i].n_vals], out[name][1], out[name][2])
@@ -537,11 +586,15 @@ class CSVInput(object):
     if il.sparse_names:
       feats['sparse_fea'] = torch.from_numpy(np.concatenate([self._ids_from_columns(n, cols) for n in il.sparse_names]))
     if il.raw_names:
-      dense = np.empty((B, il.n_dense), np.float32)
+      dense = np.zeros((B, il.n_dense), np.float32)
       for n in il.raw_names:
+        if n in _expr_features(il):
+          continue
         c0, c1 = il.raw_cols[n]
         dense[:, c0:c1] = cols[self.feature_inputs[n][0]][0].reshape(B, c1 - c0)
       feats['dense_fea'] = torch.from_numpy(dense)
+    if _expr_inputs(il):
+      feats['expr_fea'] = torch.from_numpy(np.stack([cols[f][0].astype(np.float64) for f in _expr_inputs(il)], 1))
     seq, tag = {}, {}
     for f in il.features.values():
       if f.kind not in ('seq', 'tag'):
@@ -606,6 +659,8 @@ class CSVInput(object):
     if il.raw_names:
       dense = np.zeros((len(rows), il.n_dense), np.float32)
       for n in il.raw_names:
+        if n in _expr_features(il):
+          continue
         src, sep = self.feature_inputs[n]
         c0, c1 = il.raw_cols[n]
         for i, x in enumerate(cols[src]):
@@ -613,6 +668,10 @@ class CSVInput(object):
           vals = x.split(sep) if c1 - c0 > 1 else [x]
           dense[i, c0:c0 + len(vals)] = [float(v) for v in vals[:c1 - c0]]
       feats['dense_fea'] = torch.from_numpy(dense)
+    if _expr_inputs(il):
+      feats['expr_fea'] = torch.from_numpy(np.array(
+          [[expr_number(x, f, self.ftypes[f], self.defaults.get(f)) for x in cols[f]] for f in _expr_inputs(il)],
+          np.float64).T.copy())
     seq, tag = {}, {}
     for f in il.features.values():
       if f.kind not in ('seq', 'tag'):
@@ -711,6 +770,10 @@ class ParquetInput(object):
     dc = pipeline_config.data_config
     self.weight_field = dc.sample_weight if dc.HasField('sample_weight') else None
     self.batch_size = batch_size or input_layer.batch_size
+    # (the declared types and defaults of the fields: ExprFeature inputs are read by them)
+    self.ftypes = {f.input_name: dc.DESCRIPTOR.nested_types_by_name['Field'].fields_by_name['input_type']
+                   .enum_type.values_by_number[f.input_type].name for f in dc.input_fields}
+    self.defaults = {f.input_name: f.default_val for f in dc.input_fields}
     self.feature_inputs = {}
     for fc in config_util.get_feature_configs(pipeline_config):
       name = fc.feature_name if fc.HasField('feature_name') else fc.input_names[0]
@@ -780,10 +843,28 @@ class ParquetInput(object):
     if il.raw_names:
       dense = np.zeros((n, il.n_dense), np.float32)
       for name in il.raw_names:
+        if name in _expr_features(il):
+          continue
         c0, c1 = il.raw_cols[name]
         vals, lens = self._column(table.column(self.feature_inputs[name]))
         dense[:, c0:c1] = np.asarray(vals, np.float32).reshape(n, c1 - c0)
       feats['dense_fea'] = torch.from_numpy(dense)
+    if _expr_inputs(il):
+      cols = []
+      for f in _expr_inputs(il):
+        col = table.column(f)
+        vals, lens = self._column(col)
+        t = self.ftypes.get(f, 'STRING')
+        if lens is not None:
+          raise ValueError('ExprFeature input column %r holds lists' % f)
+        if np.asarray(vals).dtype.kind in 'OUS':
+          vals = [expr_number('' if v is None else str(v), f, t, self.defaults.get(f)) for v in vals]
+        v = np.asarray(vals, np.float32 if t == 'FLOAT' else np.float64).astype(np.float64)
+        nulls = col.is_null().to_numpy(zero_copy_only=False)
+        if nulls.any():   # a null is an empty value: the field's default
+          v[nulls] = expr_number('', f, t, self.defaults.get(f))
+        cols.append(v)
+      feats['expr_fea'] = torch.from_numpy(np.stack(cols, 1))
     seq, tag = {}, {}
     for f in il.features.values():
       if f.kind not in ('seq', 'tag'):

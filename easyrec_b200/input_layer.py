@@ -28,6 +28,7 @@ import torch
 
 from easyrec_b200 import _lib
 from easyrec_b200 import embedding as E
+from easyrec_b200 import expr as X
 from easyrec_b200 import kernels as K
 
 FeatureSpec = collections.namedtuple(
@@ -36,8 +37,9 @@ FeatureSpec = collections.namedtuple(
      'embedding_dim', 'bucket_mode', 'num_buckets', 'combiner', 'embedding_name',
      'min_val', 'max_val', 'raw_input_dim', 'seq_len',
      'kv_capacity',             # > 0: a key-value table (ev_params) of that many rows per rank
+     'expr',                    # an ExprFeature: (expr.Program, its input field names), a raw column it fills
      'vocab'],                  # a vocabulary column: the 63-bit key of each entry, entry i = row i (else None)
-    defaults=(0, None))
+    defaults=(0, None, None))
 
 
 def _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed=False, vocab=None):
@@ -72,7 +74,7 @@ def id_feature(name, embedding_dim, hash_bucket_size=0, num_buckets=0, combiner=
   hash_bucket_size, num_buckets = _kv_buckets(hash_bucket_size, num_buckets, kv_capacity)
   mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed, vocab)
   return FeatureSpec(name, 'id', embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1, 1, int(kv_capacity),
-                     _vocab_tuple(vocab))
+                     vocab=_vocab_tuple(vocab))
 
 
 def _vocab_tuple(vocab):
@@ -98,7 +100,7 @@ def multi_feature(name, kind, embedding_dim, hash_bucket_size=0, num_buckets=0, 
   hash_bucket_size, num_buckets = _kv_buckets(hash_bucket_size, num_buckets, kv_capacity)
   mode, nb = _bucket_rule(hash_bucket_size, num_buckets, packed_mod, host_hashed, vocab)
   return FeatureSpec(name, kind, embedding_dim, mode, nb, combiner, embedding_name, 0., 0., 1,
-                     max(int(seq_len), 1), int(kv_capacity), _vocab_tuple(vocab))
+                     max(int(seq_len), 1), int(kv_capacity), vocab=_vocab_tuple(vocab))
 
 
 _COMBINER = {'sum': _lib.COMBINER_SUM, 'mean': _lib.COMBINER_MEAN, 'sqrtn': _lib.COMBINER_SQRTN}
@@ -220,6 +222,19 @@ class InputLayer(object):
       self.raw_cols[n] = (c, c + self.features[n].raw_input_dim)
       c += self.features[n].raw_input_dim
     self.n_dense = c
+    # ExprFeatures: their distinct input fields are the columns of features['expr_fea'], float64 [B, n]; er_expr_eval
+    # writes each expression's value into its raw column of dense_fea
+    exprs = [f for f in features if f.expr is not None]
+    self.expr_inputs = list(collections.OrderedDict((n, None) for f in exprs for n in f.expr[1]))
+    self.expr_plan = None
+    if exprs:
+      progs = []
+      for f in exprs:
+        prog, names = f.expr
+        glob = [self.expr_inputs.index(n) for n in names]
+        progs.append(prog._replace(ops=tuple((op, glob[a] if op == X.EXPR_LOAD else 0, v) for op, a, v in prog.ops)))
+      self.expr_plan = K.expr_plan(progs, [self.raw_cols[f.name][0] for f in exprs], len(self.expr_inputs), device)
+    self._expr_batch = None   # the batch whose ExprFeatures precompute_rows evaluated
     # ---- table plan -------------------------------------------------------------------
     # arenas are keyed by their dim; a key-value table has an arena of its own, keyed (dim, table)
     self.arenas = collections.OrderedDict()          # arena key -> Arena
@@ -712,7 +727,8 @@ class InputLayer(object):
     """K1 (index hashing / bucketing) of the single-valued slots at the head of the step, ahead of the lookup:
     data-parallel training all-gathers the rows and starts the global dedup sort while the dense forward/backward
     runs.  Returns [(arena dim, ArenaCall, rows, weights)]; the next lookup() reuses them."""
-    dense = features.get('dense_fea')
+    dense = self._dense_block(features)
+    self._expr_batch = features
     dense_norm = self.normalize_dense(dense) if dense is not None else None
     out = []
     self._preset_rows = {}
@@ -748,6 +764,16 @@ class InputLayer(object):
     with torch.cuda.stream(self._side):
       for m, rows, w, outs, seg_ids in self._pending:
         self.placements.presort(rows, m.arena.n_rows, m.arena.dim, m.ws, m.slots_dev, m.n_slots, seg_ids=seg_ids)
+
+  def _dense_block(self, features):
+    """features['dense_fea'] with the ExprFeature columns evaluated into it (one er_expr_eval launch)"""
+    dense = features.get('dense_fea')
+    if self.expr_plan is not None:
+      if 'expr_fea' not in features:
+        raise ValueError('the batch has no expr_fea: ExprFeatures %s read the float64 fields %s'
+                         % ([n for n, f in self.features.items() if f.expr is not None], self.expr_inputs))
+      K.expr_eval(self.expr_plan, features['expr_fea'], dense)
+    return dense
 
   def normalize_dense(self, dense):
     if self.raw_has_range:
@@ -1049,7 +1075,8 @@ class InputLayer(object):
   def lookup(self, features):
     """Runs K1 + K2 for every arena; returns {group: (concat, [per-feature views])} and fills
     self.seq_outputs {seq group: {key, hist_seq_emb, hist_seq_len}}."""
-    dense = features.get('dense_fea')
+    dense = features.get('dense_fea') if self._expr_batch is features else self._dense_block(features)
+    self._expr_batch = None
     dense_norm = self.normalize_dense(dense) if dense is not None else None
     self._rows_cache = dict(self._preset_rows)   # K1 results computed ahead of the step (precompute_rows)
     self._preset_rows = {}

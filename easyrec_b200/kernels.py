@@ -5,11 +5,12 @@ call into liber_b200.so.  Shapes/dtypes are checked on the host; nothing falls
 back to a torch implementation.
 """
 import ctypes
+import os
 
 import numpy as np
 import torch
 
-from easyrec_b200 import _lib
+from easyrec_b200 import _lib, expr
 from easyrec_b200._lib import ErOpt, SLOT_DTYPE, c_vp
 
 
@@ -331,6 +332,62 @@ def auc_hist(probs, labels, thresholds, hist):
   _lib.check(_lib.load().er_auc_hist(_p(probs), _p(labels), probs.numel(), _p(thresholds), thresholds.numel(), _p(hist),
                                      _stream()), 'er_auc_hist')
   return hist
+
+
+class ExprPlan(object):
+  """The programs of a model's ExprFeatures (expr.Program) packed for er_expr_eval: one device array holding their
+  er_expr_t descriptors, then their er_expr_op_t ops; out_cols[e] is the dense_fea column of expression e.  Each program
+  is checked on the host: its opcodes, its input indices against n_inputs and the stack it needs."""
+
+  def __init__(self, programs, out_cols, n_inputs, device):
+    self.n_expr, self.n_inputs = len(programs), int(n_inputs)
+    self.n_ops = sum(len(p.ops) for p in programs)
+    self.max_depth = max([p.depth for p in programs] + [0])
+    if self.n_ops > _lib.EXPR_MAX_OPS or self.max_depth > _lib.EXPR_MAX_STACK:
+      raise _lib.ErError('ExprFeature programs: %d ops and a stack of %d, at most %d and %d'
+                         % (self.n_ops, self.max_depth, _lib.EXPR_MAX_OPS, _lib.EXPR_MAX_STACK))
+    desc = np.zeros(self.n_expr, dtype=_lib.EXPR_DTYPE)
+    ops = np.zeros(self.n_ops, dtype=_lib.EXPR_OP_DTYPE)
+    k = 0
+    for e, (p, col) in enumerate(zip(programs, out_cols)):
+      desc[e] = (k, len(p.ops), col, 0)
+      depth = 0
+      for op, arg, value in p.ops:
+        pushes = op in (expr.EXPR_LOAD, expr.EXPR_CONST)
+        if not 0 <= op <= expr.EXPR_OR or (op == expr.EXPR_LOAD and not 0 <= arg < self.n_inputs):
+          raise _lib.ErError('ExprFeature program %d: op %d with input %d of %d' % (e, op, arg, self.n_inputs))
+        depth += 1 if pushes else (0 if op == expr.EXPR_NEG else -1)
+        if depth < 1 or depth > p.depth:
+          raise _lib.ErError('ExprFeature program %d: its stack leaves [1, %d]' % (e, p.depth))
+        ops[k] = (op, arg if op == expr.EXPR_LOAD else 0, value)
+        k += 1
+      if depth != 1:
+        raise _lib.ErError('ExprFeature program %d leaves %d values' % (e, depth))
+    blob = np.concatenate([desc.view(np.uint8), ops.view(np.uint8)]).view(np.int64)
+    self.dev = torch.from_numpy(blob.copy()).to(device)
+
+
+def expr_plan(programs, out_cols, n_inputs, device):
+  """ExprPlan on the device.  er_expr_eval runs on the GPU only, so a host device is refused (a plan built with
+  ER_PLAN_ONLY=1 only to be inspected is packed all the same)."""
+  if not str(device).startswith('cuda') and os.environ.get('ER_PLAN_ONLY') != '1':
+    raise NotImplementedError('ExprFeature columns are evaluated by er_expr_eval on the GPU; device %s has none' % device)
+  return ExprPlan(programs, out_cols, n_inputs, device)
+
+
+def expr_eval(plan, inputs, dense):
+  """er_expr_eval: inputs float64 [B, n_inputs] -> each ExprFeature's float32 value into its column of dense
+  float32 [B, n_dense], in place."""
+  _chk(inputs, torch.float64, 'expr inputs')
+  _chk(dense, torch.float32, 'dense_fea')
+  B = dense.shape[0]
+  if inputs.dim() != 2 or inputs.shape[0] != B or inputs.shape[1] != plan.n_inputs:
+    raise _lib.ErError('expr inputs must be float64 [%d, %d], got %s' % (B, plan.n_inputs, tuple(inputs.shape)))
+  base = plan.dev.data_ptr()
+  _lib.check(_lib.load().er_expr_eval(_p(inputs), B, plan.n_inputs, base, plan.n_expr, base + 16 * plan.n_expr,
+                                      plan.n_ops, plan.max_depth, _p(dense), dense.shape[1], _stream()),
+             'er_expr_eval')
+  return dense
 
 
 def binary_maps(slot_cols, raw_cols, device):

@@ -691,7 +691,11 @@ enum {
                             * inner_sep, the values of one step by kv_sep.  out int64[list_cap] = the values of all
                             * steps back to back, lens[r] = steps of line r (the first `width` non-empty ones),
                             * step_lens int32[max_rows * width] = values per step (0 beyond lens[r]) */
-  ER_CSV_HASH_STEP_LIST = 11 /* the same with fingerprinted string values */
+  ER_CSV_HASH_STEP_LIST = 11, /* the same with fingerprinted string values */
+  ER_CSV_F64 = 12          /* out double[max_rows]: a decimal number (strtod on the field without its surrounding
+                            * spaces / tabs; hex spellings are refused), an ExprFeature input read from a STRING or
+                            * DOUBLE field (tf.string_to_number(.., tf.float64), input/input.py:513-523).  An empty
+                            * field parses default_str instead; NULL or "" there makes an empty field invalid */
 };
 typedef struct {
   int32_t kind;
@@ -740,6 +744,40 @@ int er_fingerprint64_i64(const int64_t* values, int64_t n, uint64_t* out);
 int er_binary_unpack(const int32_t* label, const float* dense, const uint32_t* cat, int64_t batch,
                      const int32_t* slot_cols, int32_t n_slot, const int32_t* raw_cols, int32_t n_raw,
                      int64_t* sparse_fea, float* dense_fea, float* labels, er_stream_t stream);
+
+/* ---- ExprFeature columns (input/input.py:507-535, utils/expr_util.py) ----
+ * Each expression of a model is a postfix program over the float64 inputs of one sample, compiled on the host
+ * (easyrec_b200/expr.py).  An op pushes an input (ER_EXPR_LOAD, arg = input index) or a constant (ER_EXPR_CONST, value),
+ * negates the top (ER_EXPR_NEG), or pops two values a (below) and b (top) and pushes a op b: + - * / in float64
+ * rounded to nearest, the five comparisons and & / | (operands 0.0 = false, else true) as 1.0 / 0.0. */
+#define ER_EXPR_MAX_STACK 8      /* values on the evaluation stack */
+#define ER_EXPR_MAX_OPS 4096     /* ops of all the programs of one call */
+enum {
+  ER_EXPR_LOAD = 0, ER_EXPR_CONST = 1, ER_EXPR_ADD = 2, ER_EXPR_SUB = 3, ER_EXPR_MUL = 4, ER_EXPR_DIV = 5,
+  ER_EXPR_NEG = 6, ER_EXPR_GT = 7, ER_EXPR_GE = 8, ER_EXPR_LT = 9, ER_EXPR_LE = 10, ER_EXPR_EQ = 11,
+  ER_EXPR_AND = 12, ER_EXPR_OR = 13
+};
+typedef struct {
+  int32_t op;
+  int32_t arg;
+  double value;
+} er_expr_op_t;          /* 16 bytes */
+typedef struct {
+  int32_t begin;         /* first op of the program in the ops array */
+  int32_t n_ops;
+  int32_t out_col;       /* the column of dense the result goes to */
+  int32_t pad_;
+} er_expr_t;             /* 16 bytes */
+/* dense[b * dense_pitch + exprs[e].out_col] = (float) (value of program e on inputs[b * n_inputs ...]) for every sample
+ * b < batch and expression e < n_expr: one launch, one thread per (expression, sample).  inputs float64[batch,
+ * n_inputs], exprs er_expr_t[n_expr] and ops er_expr_op_t[n_ops] are DEVICE arrays (exprs and ops may be one
+ * allocation).  max_depth: the deepest stack any program needs, at most ER_EXPR_MAX_STACK; a program that goes deeper
+ * loses its bottom values.  The kernel reads only inside the arrays it is given whatever they hold: an input index
+ * outside [0, n_inputs) reads NaN, a program reaching past n_ops runs no op, an out_col outside [0, dense_pitch) writes
+ * nothing.  No allocation, no synchronisation; capturable in a CUDA graph. */
+int er_expr_eval(const double* inputs, int64_t batch, int32_t n_inputs, const er_expr_t* exprs, int32_t n_expr,
+                 const er_expr_op_t* ops, int32_t n_ops, int32_t max_depth, float* dense, int64_t dense_pitch,
+                 er_stream_t stream);
 
 /* ---- sharded-table restore: the LoadEmbed custom op (ops/src/load_dense_embed.cc:28-156;
  * python fallback compat/embedding_parallel_saver.py:141-173) ----
